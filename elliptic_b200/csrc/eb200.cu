@@ -10,6 +10,7 @@
 #include <cstdlib>
 #include <mutex>
 #include <thread>
+#include <type_traits>
 #include <vector>
 #include "../../include/elliptic_b200.h"
 #include "ecdsa_k256_body.cuh"
@@ -18,11 +19,6 @@
 #include "ecdsa_k256_sign_fast.cuh"
 #include "der_sig.cuh"
 #include "ecdsa_sw_sign.cuh"
-
-// Calls F(curve-parameter type) for the non-GLV short curve `curve`.
-#define SW_DISPATCH(curve, F)                                                                    \
-  ((curve) == EB200_CURVE_P256 ? F(P256) : (curve) == EB200_CURVE_P384 ? F(P384) :               \
-   (curve) == EB200_CURVE_P521 ? F(P521) : (curve) == EB200_CURVE_P192 ? F(P192) : F(P224))
 #include "ecdsa_k256_sign.cuh"
 #include "ecdsa_sw_body.cuh"
 #include "ed25519_body.cuh"
@@ -381,7 +377,6 @@ __global__ void __launch_bounds__(128) sw_decode_pub_kernel(size_t N, const uint
                                                             uint8_t* __restrict__ xy, uint8_t* __restrict__ pre) {
   typedef SW<C> W;
   typedef typename W::F F;
-  constexpr int NL = W::N;
   constexpr size_t LEN = C::LEN;
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
@@ -542,12 +537,10 @@ rt_curve_kernel(int op, size_t N, RtCurve<NL> C, const uint8_t* __restrict__ k1,
 // contexts: one per CUDA device, created by eb200_init(devices, ndev, flags).  Host-pointer calls are
 // sharded over the initialised devices in contiguous blocks (SURVEY 8e), each block driven by its own host
 // thread on its own device; device-pointer calls run on the device that owns the pointers.
-namespace {
-constexpr int MAX_CHUNKS = 16;
-}  // namespace
-#define EB_MAX_CHUNKS 16
 #include "chunk_plan.h"
 namespace {
+constexpr int MAX_CHUNKS = EB_MAX_CHUNKS;
+constexpr int MAX_CURVES = 16;                       // curve ids index the per-context table arrays
 constexpr int MAX_DEV = 16;
 constexpr int STAGE_SLOTS = 8;                       // pinned staging ring for pageable caller buffers
 constexpr size_t STAGE_BYTES = (size_t)4 << 20;
@@ -604,18 +597,22 @@ class CopyPool {
   bool stop_ = false;
 };
 
+// Ctx::ev slots of the single-stream and device-pointer calls: h2d_ms = START..INPUTS_RESIDENT,
+// kernel_ms = INPUTS_RESIDENT..KERNELS_DONE, d2h_ms = KERNELS_DONE..OUTPUTS_HOME, main_kernel_ms = MAIN_BEGIN..MAIN_END.
+enum { EV_START, EV_INPUTS_RESIDENT, EV_KERNELS_DONE, EV_OUTPUTS_HOME, EV_MAIN_BEGIN, EV_MAIN_END, EV_SLOTS };
+
 struct Ctx {
   std::mutex mu;                      // serialises the calls that use this device's buffers / events
   bool ready = false;
   int device = -1;
   cudaStream_t stream = nullptr, stream2 = nullptr, copy_stream = nullptr;
-  u32* gtab[16] = {};
-  u32* sw_replay_tab[16] = {};         // p256/p384: the reference's wnd-8 NAF table of G
+  u32* gtab[MAX_CURVES] = {};
+  u32* sw_replay_tab[MAX_CURVES] = {}; // p256/p384: the reference's wnd-8 NAF table of G
   u32* replay_tab = nullptr;          // secp256k1: the reference's wnd-7 NAF table of G and its beta image
   uint8_t* d_in = nullptr; size_t d_in_cap = 0;
   uint8_t* d_ws = nullptr; size_t d_ws_cap = 0;
   uint8_t* d_status = nullptr; size_t d_status_cap = 0;
-  cudaEvent_t ev[6] = {};
+  cudaEvent_t ev[EV_SLOTS] = {};
   cudaEvent_t ev_in[MAX_CHUNKS] = {}, ev_k0[MAX_CHUNKS] = {}, ev_k1[MAX_CHUNKS] = {}, ev_done[MAX_CHUNKS] = {};
   uint8_t* h_stage[STAGE_SLOTS] = {};
   cudaEvent_t ev_stage[STAGE_SLOTS] = {};
@@ -639,6 +636,67 @@ int cuda_fail(cudaError_t e, const char* what) {
   return (e == cudaErrorNoDevice || e == cudaErrorInsufficientDriver) ? EB200_ERR_NO_DEVICE : EB200_ERR_CUDA;
 }
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuda_fail(e_, #call); } while (0)
+
+// Launches kernels on one stream and counts them for eb200_timing.launches.  After a failed launch it launches
+// nothing more and keeps the error in `rc` for the caller to return.
+struct Launch {
+  cudaStream_t st;
+  unsigned count = 0;
+  int rc = EB200_OK;
+  template <class... P, class... A>
+  void operator()(void (*kernel)(P...), unsigned grid, unsigned block, A... args) {
+    if (rc) return;
+    kernel<<<grid, block, 0, st>>>(args...);
+    count++;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) rc = cuda_fail(e, "cudaGetLastError()");
+  }
+};
+unsigned blocks128(size_t threads) { return (unsigned)((threads + 127) / 128); }
+// grid of a prep / finish kernel whose threads each take up to `batch` items
+unsigned batch_blocks(size_t n, int batch) { return blocks128((n + batch - 1) / batch); }
+
+// Which kernels serve a curve id: secp256k1 and ed25519 have their own, the other short curves share the SW<C>
+// templates and sign with their curves.js hash (p384: SHA-384, p521: SHA-512, the rest: SHA-256).
+struct K256Curve {};
+struct Ed25519Curve {};
+template <class C_> struct SwCurve {
+  typedef C_ C;
+  typedef SWSign<C, std::conditional_t<std::is_same<C, P384>::value, Sha384W,
+                                       std::conditional_t<std::is_same<C, P521>::value, Sha512W, Sha256W>>> SG;
+};
+template <class T> constexpr bool is_k256 = std::is_same<T, K256Curve>::value;
+template <class T> constexpr bool is_ed25519 = std::is_same<T, Ed25519Curve>::value;
+
+// Calls f(tag) with the tag type of `curve` (f returns an int status); EB200_ERR_UNSUPPORTED for other ids.
+template <class F>
+int with_curve(int curve, F&& f) {
+  switch (curve) {
+    case EB200_CURVE_SECP256K1: return f(K256Curve{});
+    case EB200_CURVE_ED25519: return f(Ed25519Curve{});
+    case EB200_CURVE_P256: return f(SwCurve<P256>{});
+    case EB200_CURVE_P384: return f(SwCurve<P384>{});
+    case EB200_CURVE_P521: return f(SwCurve<P521>{});
+    case EB200_CURVE_P192: return f(SwCurve<P192>{});
+    case EB200_CURVE_P224: return f(SwCurve<P224>{});
+    default: return EB200_ERR_UNSUPPORTED;
+  }
+}
+
+// nvcc emits kernel templates in the order in which it first needs them, and NVVM's inlining into the 255-register
+// p521 kernels (their registers and spills) depends on that order.  The dispatch above reaches every short-curve
+// kernel through nested templates; naming these four families first keeps the module order their code was tuned in.
+[[maybe_unused]] const void* const sw_kernel_order[] = {
+    (const void*)sw_decode_pub_kernel<P256>, (const void*)sw_decode_pub_kernel<P384>, (const void*)sw_decode_pub_kernel<P521>,
+    (const void*)sw_decode_pub_kernel<P192>, (const void*)sw_decode_pub_kernel<P224>,
+    (const void*)sw_keygen_kernel<SwCurve<P256>::SG>, (const void*)sw_keygen_kernel<SwCurve<P384>::SG>,
+    (const void*)sw_keygen_kernel<SwCurve<P521>::SG>, (const void*)sw_keygen_kernel<SwCurve<P192>::SG>,
+    (const void*)sw_keygen_kernel<SwCurve<P224>::SG>,
+    (const void*)sw_mul_g_kernel<P256>, (const void*)sw_mul_g_kernel<P384>, (const void*)sw_mul_g_kernel<P521>,
+    (const void*)sw_mul_g_kernel<P192>, (const void*)sw_mul_g_kernel<P224>,
+    (const void*)sw_selftest_fe_kernel<P256>, (const void*)sw_selftest_fe_kernel<P384>, (const void*)sw_selftest_fe_kernel<P521>,
+    (const void*)sw_selftest_fe_kernel<P192>, (const void*)sw_selftest_fe_kernel<P224>,
+};
 
 int grow(uint8_t** p, size_t* cap, size_t need) {
   if (*cap >= need) return EB200_OK;
@@ -671,14 +729,14 @@ size_t pub_item_bytes(size_t len, u32 fmt) {
 // workspace: [ws words | scratch words | qtab words | decoded xy | pre-status]
 struct WsLayout { size_t ws, scratch, qtab, xy, pre, total; };
 WsLayout ws_layout(int curve, size_t n) {
-  size_t prep_words, scratch_words, qtab_words, len = curve_len(curve);
-  if (curve == EB200_CURVE_SECP256K1) { prep_words = PREP_WORDS; scratch_words = 8; qtab_words = QTAB_WORDS; }
-  else if (curve == EB200_CURVE_ED25519) { prep_words = 0; scratch_words = 0; qtab_words = ED_ATAB_WORDS; }
-  else {
-#define EB_WS(C) (prep_words = SW<C>::PREP_WORDS, scratch_words = SW<C>::N, qtab_words = SW<C>::QTAB_WORDS, 0)
-    (void)SW_DISPATCH(curve, EB_WS);
-#undef EB_WS
-  }
+  size_t prep_words = 0, scratch_words = 0, qtab_words = 0, len = curve_len(curve);
+  with_curve(curve, [&](auto cv) {
+    typedef decltype(cv) T;
+    if constexpr (is_k256<T>) { prep_words = PREP_WORDS; scratch_words = 8; qtab_words = QTAB_WORDS; }
+    else if constexpr (is_ed25519<T>) qtab_words = ED_ATAB_WORDS;
+    else { typedef SW<typename T::C> W; prep_words = W::PREP_WORDS; scratch_words = W::N; qtab_words = W::QTAB_WORDS; }
+    return EB200_OK;
+  });
   WsLayout L;
   L.ws = 0;
   L.scratch = align256(L.ws + prep_words * n * 4);
@@ -749,144 +807,90 @@ int h2d(Ctx& c, const Seg* seg, int k, cudaStream_t st) {
   }
   return EB200_OK;
 }
-int h2d1(Ctx& c, void* dst, const void* src, size_t bytes, cudaStream_t st) {
-  Seg s{dst, src, bytes};
-  return h2d(c, &s, 1, st);
-}
 
-template <class C>
-int sw_ensure_table(Ctx& c, int curve) {
-  typedef SW<C> W;
-  if (c.gtab[curve]) return EB200_OK;
-  size_t entries = (size_t)W::GWINDOWS * W::GENTRIES;
-  CK(cudaMalloc(&c.gtab[curve], entries * 2 * W::N * 4));
-  sw_gtab_kernel<C><<<(unsigned)((entries + 127) / 128), 128, 0, c.stream>>>(c.gtab[curve]);
-  CK(cudaGetLastError());
-  CK(cudaMalloc(&c.sw_replay_tab[curve], (size_t)SWReplay<C>::TAB_WORDS * 4));
-  sw_replay_tab_kernel<C><<<1, 128, 0, c.stream>>>(c.sw_replay_tab[curve]);
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(c.stream));
-  return EB200_OK;
-}
+// Builds the fixed-base table of `curve` (and the replay table of the curves that have one) on first use.
 int ensure_table(Ctx& c, int curve) {
-  if (curve == EB200_CURVE_SECP256K1) {
+  return with_curve(curve, [&](auto cv) {
+    typedef decltype(cv) T;
     if (c.gtab[curve]) return EB200_OK;
-    size_t entries = (size_t)GTAB_WINDOWS * GTAB_ENTRIES;
-    CK(cudaMalloc(&c.gtab[curve], entries * 16 * 4));
-    k256_gtab_kernel<<<(unsigned)((entries + 127) / 128), 128, 0, c.stream>>>(c.gtab[curve]);
-    CK(cudaGetLastError());
-    CK(cudaMalloc(&c.replay_tab, (size_t)REPLAY_TAB_WORDS * 4));
-    k256_replay_tab_kernel<<<2, 128, 0, c.stream>>>(c.replay_tab);
+    if constexpr (is_k256<T>) {
+      size_t entries = (size_t)GTAB_WINDOWS * GTAB_ENTRIES;
+      CK(cudaMalloc(&c.gtab[curve], entries * 16 * 4));
+      k256_gtab_kernel<<<blocks128(entries), 128, 0, c.stream>>>(c.gtab[curve]);
+      CK(cudaGetLastError());
+      CK(cudaMalloc(&c.replay_tab, (size_t)REPLAY_TAB_WORDS * 4));
+      k256_replay_tab_kernel<<<2, 128, 0, c.stream>>>(c.replay_tab);
+    } else if constexpr (is_ed25519<T>) {
+      size_t entries = (size_t)ED_GWINDOWS * ED_GENTRIES;
+      CK(cudaMalloc(&c.gtab[curve], entries * 24 * 4));
+      ed_gtab_kernel<<<blocks128(entries), 128, 0, c.stream>>>(c.gtab[curve]);
+    } else {
+      typedef typename T::C C;
+      typedef SW<C> W;
+      size_t entries = (size_t)W::GWINDOWS * W::GENTRIES;
+      CK(cudaMalloc(&c.gtab[curve], entries * 2 * W::N * 4));
+      sw_gtab_kernel<C><<<blocks128(entries), 128, 0, c.stream>>>(c.gtab[curve]);
+      CK(cudaGetLastError());
+      CK(cudaMalloc(&c.sw_replay_tab[curve], (size_t)SWReplay<C>::TAB_WORDS * 4));
+      sw_replay_tab_kernel<C><<<1, 128, 0, c.stream>>>(c.sw_replay_tab[curve]);
+    }
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(c.stream));
     return EB200_OK;
-  }
-  if (curve == EB200_CURVE_P256 || curve == EB200_CURVE_P384 || curve == EB200_CURVE_P521 || curve == EB200_CURVE_P192 ||
-      curve == EB200_CURVE_P224) {
-#define EB_ENS(C) sw_ensure_table<C>(c, curve)
-    return SW_DISPATCH(curve, EB_ENS);
-#undef EB_ENS
-  }
-  if (curve == EB200_CURVE_ED25519) {
-    if (c.gtab[curve]) return EB200_OK;
-    size_t entries = (size_t)ED_GWINDOWS * ED_GENTRIES;
-    CK(cudaMalloc(&c.gtab[curve], entries * 24 * 4));
-    ed_gtab_kernel<<<(unsigned)((entries + 127) / 128), 128, 0, c.stream>>>(c.gtab[curve]);
-    CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(c.stream));
-    return EB200_OK;
-  }
-  return EB200_ERR_UNSUPPORTED;
+  });
 }
 
-template <class C>
-int sw_launch_verify(Ctx& c, int curve, size_t n, const uint8_t* d_e, const uint8_t* d_r, const uint8_t* d_s, const uint8_t* xy,
-                     const uint8_t* pre, u32* ws, u32* scratch, u32* qtab, uint8_t* d_status, cudaStream_t st,
-                     unsigned pb, unsigned nb, cudaEvent_t ev_main0, cudaEvent_t* ev_main1) {
-  sw_prep_kernel<C><<<pb, 128, 0, st>>>(n, d_e, d_r, d_s, ws, scratch);
-  CK(cudaGetLastError());
-  if (ev_main0) CK(cudaEventRecord(ev_main0, st));
-  sw_verify_kernel<C><<<nb, 128, 0, st>>>(n, xy, d_r, ws, c.gtab[curve], qtab, pre, d_status);
-  CK(cudaGetLastError());
-  if (*ev_main1) { CK(cudaEventRecord(*ev_main1, st)); *ev_main1 = nullptr; }
-  sw_replay_kernel<C><<<nb, 128, 0, st>>>(n, d_e, d_r, d_s, xy, c.sw_replay_tab[curve], d_status);
-  return EB200_OK;
-}
-
-// Launches decode (if needed) + prep + verify for n items on stream st.  All pointers are device pointers.
+// Launches decode (if needed) + prep + verify for n items on L's stream, recording ev_main0 / ev_main1 around the
+// main kernel.  All pointers are device pointers.
 int launch_verify(Ctx& c, int curve, size_t n, const uint8_t* d_e, const uint8_t* d_r, const uint8_t* d_s,
-                  const uint8_t* d_pub, u32 pub_fmt, uint8_t* d_status, uint8_t* d_workspace,
-                  cudaStream_t st, cudaEvent_t ev_main0, cudaEvent_t ev_main1, unsigned* launches,
+                  const uint8_t* d_pub, u32 pub_fmt, uint8_t* d_status, uint8_t* d_workspace, Launch& L,
+                  cudaEvent_t ev_main0, cudaEvent_t ev_main1,
                   const uint8_t* d_der = nullptr, const unsigned long long* d_der_off = nullptr) {
   if (n == 0) return EB200_OK;
-  WsLayout L = ws_layout(curve, n);
-  u32* ws = (u32*)(d_workspace + L.ws);
-  u32* scratch = (u32*)(d_workspace + L.scratch);
-  u32* qtab = (u32*)(d_workspace + L.qtab);
+  const WsLayout W = ws_layout(curve, n);
+  u32* ws = (u32*)(d_workspace + W.ws);
+  u32* scratch = (u32*)(d_workspace + W.scratch);
+  u32* qtab = (u32*)(d_workspace + W.qtab);
+  uint8_t* dxy = d_workspace + W.xy;
+  uint8_t* dpre = d_workspace + W.pre;
   const uint8_t* xy = d_pub;
   const uint8_t* pre = nullptr;
-  unsigned nb = (unsigned)((n + 127) / 128);
-  size_t T = (n + PREP_BATCH - 1) / PREP_BATCH;
-  unsigned pb = (unsigned)((T + 127) / 128);
-  unsigned cnt = 0;
-  if (curve == EB200_CURVE_ED25519) {       // the `ec` API over the Edwards preset: one kernel, per-item scalar inversion
+  const unsigned nb = blocks128(n);
+  const u32* gt = c.gtab[curve];
+  return with_curve(curve, [&](auto cv) {
+    typedef decltype(cv) T;
     if (pub_fmt != EB200_PUB_XY) {
-      ed_ec_decode_pub_kernel<<<nb, 128, 0, st>>>(n, d_pub, pub_fmt, d_workspace + L.xy, d_workspace + L.pre);
-      CK(cudaGetLastError());
-      xy = d_workspace + L.xy; pre = d_workspace + L.pre; cnt++;
+      if constexpr (is_k256<T>) L(k256_decode_pub_kernel, nb, 128, n, d_pub, pub_fmt, dxy, dpre);
+      else if constexpr (is_ed25519<T>) L(ed_ec_decode_pub_kernel, nb, 128, n, d_pub, pub_fmt, dxy, dpre);
+      else L(sw_decode_pub_kernel<typename T::C>, nb, 128, n, d_pub, pub_fmt, dxy, dpre);
+      xy = dxy; pre = dpre;
     }
-    if (d_der) {
-      der_decode_kernel<<<nb, 128, 0, st>>>(n, 32u, d_der, d_der_off, (uint8_t*)d_r, (uint8_t*)d_s, d_workspace + L.pre, pre != nullptr);
-      CK(cudaGetLastError());
-      pre = d_workspace + L.pre; cnt++;
+    if (d_der) {     // d_r / d_s are then scratch the decoder fills
+      L(der_decode_kernel, nb, 128, n, (u32)curve_len(curve), d_der, d_der_off, (uint8_t*)d_r, (uint8_t*)d_s, dpre,
+        (int)(pre != nullptr));
+      pre = dpre;
     }
-    if (ev_main0) CK(cudaEventRecord(ev_main0, st));
-    ed_ec_verify_kernel<<<nb, 128, 0, st>>>(n, d_e, d_r, d_s, xy, pre, c.gtab[curve], qtab, d_status);
-    CK(cudaGetLastError());
-    if (ev_main1) CK(cudaEventRecord(ev_main1, st));
-    if (launches) *launches += cnt + 1;
-    return EB200_OK;
-  }
-  if (pub_fmt != EB200_PUB_XY) {
-    uint8_t* dxy = d_workspace + L.xy;
-    uint8_t* dpre = d_workspace + L.pre;
-    if (curve == EB200_CURVE_SECP256K1) k256_decode_pub_kernel<<<nb, 128, 0, st>>>(n, d_pub, pub_fmt, dxy, dpre);
-    else {
-#define EB_DEC(C) (sw_decode_pub_kernel<C><<<nb, 128, 0, st>>>(n, d_pub, pub_fmt, dxy, dpre), 0)
-      (void)SW_DISPATCH(curve, EB_DEC);
-#undef EB_DEC
+    if constexpr (is_ed25519<T>) {     // the `ec` API over the Edwards preset: one kernel, per-item scalar inversion
+      CK(cudaEventRecord(ev_main0, L.st));
+      L(ed_ec_verify_kernel, nb, 128, n, d_e, d_r, d_s, xy, pre, gt, qtab, d_status);
+      CK(cudaEventRecord(ev_main1, L.st));
+    } else if constexpr (is_k256<T>) {
+      L(k256_prep_kernel, batch_blocks(n, PREP_BATCH), 128, n, d_e, d_r, d_s, ws, scratch);
+      CK(cudaEventRecord(ev_main0, L.st));
+      L(k256_verify_kernel, (unsigned)((n + EB_VERIFY_BLOCK - 1) / EB_VERIFY_BLOCK), EB_VERIFY_BLOCK, n, xy, d_r, ws, gt,
+        qtab, pre, d_status);
+      CK(cudaEventRecord(ev_main1, L.st));
+      L(k256_replay_kernel, nb, 128, n, d_e, d_r, d_s, xy, c.replay_tab, d_status);
+    } else {
+      typedef typename T::C C;
+      L(sw_prep_kernel<C>, batch_blocks(n, SW<C>::BATCH), 128, n, d_e, d_r, d_s, ws, scratch);
+      CK(cudaEventRecord(ev_main0, L.st));
+      L(sw_verify_kernel<C>, nb, 128, n, xy, d_r, ws, gt, qtab, pre, d_status);
+      CK(cudaEventRecord(ev_main1, L.st));
+      L(sw_replay_kernel<C>, nb, 128, n, d_e, d_r, d_s, xy, c.sw_replay_tab[curve], d_status);
     }
-    CK(cudaGetLastError());
-    xy = dxy; pre = dpre; cnt++;
-  }
-  if (d_der) {     // d_r / d_s are then scratch the decoder fills
-    uint8_t* dpre = d_workspace + L.pre;
-    der_decode_kernel<<<nb, 128, 0, st>>>(n, (u32)curve_len(curve), d_der, d_der_off, (uint8_t*)d_r, (uint8_t*)d_s, dpre, pre != nullptr);
-    CK(cudaGetLastError());
-    pre = dpre; cnt++;
-  }
-  if (curve == EB200_CURVE_SECP256K1) {
-    k256_prep_kernel<<<pb, 128, 0, st>>>(n, d_e, d_r, d_s, ws, scratch);
-    CK(cudaGetLastError());
-    if (ev_main0) CK(cudaEventRecord(ev_main0, st));
-    unsigned vb = (unsigned)((n + EB_VERIFY_BLOCK - 1) / EB_VERIFY_BLOCK);
-    k256_verify_kernel<<<vb, EB_VERIFY_BLOCK, 0, st>>>(n, xy, d_r, ws, c.gtab[curve], qtab, pre, d_status);
-    CK(cudaGetLastError());
-    if (ev_main1) { CK(cudaEventRecord(ev_main1, st)); ev_main1 = nullptr; }
-    k256_replay_kernel<<<nb, 128, 0, st>>>(n, d_e, d_r, d_s, xy, c.replay_tab, d_status);
-    cnt++;
-  } else {
-#define EB_VER(C) sw_launch_verify<C>(c, curve, n, d_e, d_r, d_s, xy, pre, ws, scratch, qtab, d_status, st, pb, nb, ev_main0, &ev_main1)
-    int rc = SW_DISPATCH(curve, EB_VER);
-#undef EB_VER
-    if (rc) return rc;
-    cnt++;
-  }
-  CK(cudaGetLastError());
-  if (ev_main1) CK(cudaEventRecord(ev_main1, st));
-  cnt += 2;
-  if (launches) *launches += cnt;
-  return EB200_OK;
+    return L.rc;
+  });
 }
 
 bool curve_ok(int curve) { return curve_len(curve) != 0; }
@@ -898,7 +902,7 @@ int ctx_create(Ctx& c, int device) {
   CK(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
   CK(cudaStreamCreateWithFlags(&c.copy_stream, cudaStreamNonBlocking));
   CK(cudaStreamCreateWithFlags(&c.stream2, cudaStreamNonBlocking));
-  for (int i = 0; i < 6; i++) CK(cudaEventCreate(&c.ev[i]));
+  for (int i = 0; i < EV_SLOTS; i++) CK(cudaEventCreate(&c.ev[i]));
   for (int i = 0; i < MAX_CHUNKS; i++) {
     CK(cudaEventCreate(&c.ev_in[i]));
     CK(cudaEventCreate(&c.ev_k0[i]));
@@ -912,14 +916,14 @@ void ctx_destroy(Ctx& c) {
   if (c.device < 0) return;
   cudaSetDevice(c.device);
   if (c.stream) cudaStreamSynchronize(c.stream);
-  for (int k = 0; k < 16; k++) if (c.gtab[k]) { cudaFree(c.gtab[k]); c.gtab[k] = nullptr; }
-  for (int k = 0; k < 16; k++) if (c.sw_replay_tab[k]) { cudaFree(c.sw_replay_tab[k]); c.sw_replay_tab[k] = nullptr; }
+  for (int k = 0; k < MAX_CURVES; k++) if (c.gtab[k]) { cudaFree(c.gtab[k]); c.gtab[k] = nullptr; }
+  for (int k = 0; k < MAX_CURVES; k++) if (c.sw_replay_tab[k]) { cudaFree(c.sw_replay_tab[k]); c.sw_replay_tab[k] = nullptr; }
   if (c.replay_tab) { cudaFree(c.replay_tab); c.replay_tab = nullptr; }
   // the staging buffers may hold private keys or nonces of a signing call: wipe before release
   if (c.d_in) { cudaMemset(c.d_in, 0, c.d_in_cap); cudaFree(c.d_in); } c.d_in = nullptr; c.d_in_cap = 0;
   if (c.d_ws) { cudaMemset(c.d_ws, 0, c.d_ws_cap); cudaFree(c.d_ws); } c.d_ws = nullptr; c.d_ws_cap = 0;
   cudaFree(c.d_status); c.d_status = nullptr; c.d_status_cap = 0;
-  for (int i = 0; i < 6; i++) if (c.ev[i]) { cudaEventDestroy(c.ev[i]); c.ev[i] = nullptr; }
+  for (int i = 0; i < EV_SLOTS; i++) if (c.ev[i]) { cudaEventDestroy(c.ev[i]); c.ev[i] = nullptr; }
   for (int i = 0; i < MAX_CHUNKS; i++) {
     if (c.ev_in[i]) { cudaEventDestroy(c.ev_in[i]); c.ev_in[i] = nullptr; }
     if (c.ev_k0[i]) { cudaEventDestroy(c.ev_k0[i]); c.ev_k0[i] = nullptr; }
@@ -1007,6 +1011,116 @@ int run_sharded(size_t n, F&& fn) {
   t_timing = tm;
   return rc;
 }
+
+// A device -> host copy; rows > 1: `rows` rows of `bytes`, `pitch` bytes apart on the device, packed on the host.
+// A NULL destination (an output the caller did not ask for) is skipped.
+struct OutSeg { void* dst; const void* src; size_t bytes; size_t rows = 1, pitch = 0; };
+struct Wipe { void* dst; size_t bytes; };
+
+// Single-stream host call on c.stream: the inputs go up, run(L) launches the kernels, the outputs come home, and
+// the device ranges in `wipe` (private keys, nonces) are cleared before the call returns.  kernel_ms covers the
+// kernels only; main_kernel_ms is the same span when main_is_total, else the MAIN_BEGIN..MAIN_END events run records.
+template <class Run>
+int run_single(Ctx& c, std::initializer_list<Seg> in, Run&& run, std::initializer_list<OutSeg> out,
+               std::initializer_list<Wipe> wipe, bool main_is_total) {
+  cudaStream_t st = c.stream;
+  Launch L{st};
+  int rc;
+  CK(cudaEventRecord(c.ev[EV_START], st));
+  if ((rc = h2d(c, in.begin(), (int)in.size(), st))) return rc;
+  CK(cudaEventRecord(c.ev[EV_INPUTS_RESIDENT], st));
+  if ((rc = run(L)) || (rc = L.rc)) return rc;
+  CK(cudaEventRecord(c.ev[EV_KERNELS_DONE], st));
+  for (const OutSeg& o : out) {
+    if (!o.dst || !o.bytes) continue;
+    if (o.rows > 1) CK(cudaMemcpy2DAsync(o.dst, o.bytes, o.src, o.pitch, o.bytes, o.rows, cudaMemcpyDeviceToHost, st));
+    else CK(cudaMemcpyAsync(o.dst, o.src, o.bytes, cudaMemcpyDeviceToHost, st));
+  }
+  for (const Wipe& w : wipe) if (w.bytes) CK(cudaMemsetAsync(w.dst, 0, w.bytes, st));
+  CK(cudaEventRecord(c.ev[EV_OUTPUTS_HOME], st));
+  CK(cudaStreamSynchronize(st));
+  cudaEventElapsedTime(&c.timing.h2d_ms, c.ev[EV_START], c.ev[EV_INPUTS_RESIDENT]);
+  cudaEventElapsedTime(&c.timing.kernel_ms, c.ev[EV_INPUTS_RESIDENT], c.ev[EV_KERNELS_DONE]);
+  cudaEventElapsedTime(&c.timing.d2h_ms, c.ev[EV_KERNELS_DONE], c.ev[EV_OUTPUTS_HOME]);
+  if (main_is_total) c.timing.main_kernel_ms = c.timing.kernel_ms;
+  else cudaEventElapsedTime(&c.timing.main_kernel_ms, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
+  c.timing.launches = L.count;
+  return EB200_OK;
+}
+
+// Two-stream chunk pipeline of the fixed-stride host calls: chunk k's inputs go up on the copy stream, its kernels
+// run on stream (k & 1) (so the grid tail of one chunk is filled by the next), its outputs come home on the copy
+// stream behind them.  in(lo, m, seg) / out(lo, m, seg) fill up to 8 segments (out: dst = host, src = device);
+// run(lo, m, L, slot, k) launches the kernels through L and records ev_k0[k] / ev_k1[k] around the main one.
+// kernel_ms is the whole call on the GPU timeline; main_kernel_ms the span of the main kernels.
+template <class In, class Run, class Out>
+int run_chunked(Ctx& c, const ChunkPlan& P, In&& in, Run&& run, Out&& out) {
+  int rc;
+  cudaStream_t cs = c.copy_stream;
+  unsigned launches = 0;
+  CK(cudaEventRecord(c.ev[EV_START], cs));
+  int used = 0;
+  for (int k = 0; k < P.chunks; k++) {
+    size_t lo = P.lo[k];
+    size_t m = P.lo[k + 1] - lo;
+    used = k + 1;
+    Seg seg[8];
+    int cnt = in(lo, m, seg);
+    if ((rc = h2d(c, seg, cnt, cs))) return rc;
+    CK(cudaEventRecord(c.ev_in[k], cs));
+    Launch L{(k & 1) ? c.stream2 : c.stream};
+    CK(cudaStreamWaitEvent(L.st, c.ev_in[k], 0));
+    if ((rc = run(lo, m, L, k & 1, k)) || (rc = L.rc)) return rc;
+    launches += L.count;
+    CK(cudaEventRecord(c.ev_done[k], L.st));
+  }
+  for (int k = 0; k < used; k++) {
+    size_t lo = P.lo[k];
+    size_t m = P.lo[k + 1] - lo;
+    CK(cudaStreamWaitEvent(cs, c.ev_done[k], 0));
+    Seg seg[8];
+    int cnt = out(lo, m, seg);
+    for (int j = 0; j < cnt; j++)
+      if (seg[j].dst && seg[j].bytes) CK(cudaMemcpyAsync(seg[j].dst, seg[j].src, seg[j].bytes, cudaMemcpyDeviceToHost, cs));
+  }
+  CK(cudaEventRecord(c.ev[EV_OUTPUTS_HOME], cs));
+  CK(cudaStreamSynchronize(cs));
+  CK(cudaStreamSynchronize(c.stream));
+  CK(cudaStreamSynchronize(c.stream2));
+  float total = 0, t = 0;
+  cudaEventElapsedTime(&total, c.ev[EV_START], c.ev[EV_OUTPUTS_HOME]);
+  cudaEventElapsedTime(&c.timing.h2d_ms, c.ev[EV_START], c.ev_in[used - 1]);       // all inputs resident
+  for (int k = 0; k < used; k++) {       // chunks overlap on two streams: report the span of the main kernels
+    cudaEventElapsedTime(&t, c.ev_k0[0], c.ev_k1[k]);
+    if (t > c.timing.main_kernel_ms) c.timing.main_kernel_ms = t;
+  }
+  cudaEventElapsedTime(&t, c.ev_done[used - 1], c.ev[EV_OUTPUTS_HOME]);
+  c.timing.d2h_ms = t;                                                              // exposed tail copy
+  c.timing.kernel_ms = total;
+  c.timing.launches = launches;
+  return EB200_OK;
+}
+
+// Device-pointer call on the context that owns d_status (and the fixed-base table of `table_curve`, 0 = none): the
+// kernels go on the caller's stream between the INPUTS_RESIDENT and KERNELS_DONE events, which
+// eb200_last_timing() reads once the caller has synchronised that stream.
+template <class Run>
+int run_dev(const void* d_status, int table_curve, void* stream, Run&& run) {
+  Ctx* cp = ctx_of(d_status);
+  if (!cp) return EB200_ERR_NOT_INIT;
+  Ctx& c = *cp;
+  std::lock_guard<std::mutex> lk(c.mu);
+  CK(cudaSetDevice(c.device));
+  int rc;
+  if (table_curve && (rc = ensure_table(c, table_curve))) return rc;
+  Launch L{(cudaStream_t)stream};   // NULL is the CUDA default stream, as everywhere in CUDA
+  CK(cudaEventRecord(c.ev[EV_INPUTS_RESIDENT], L.st));
+  if ((rc = run(c, L)) || (rc = L.rc)) return rc;
+  CK(cudaEventRecord(c.ev[EV_KERNELS_DONE], L.st));
+  t_pending = &c;
+  t_pending_launches = L.count;
+  return EB200_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -1082,8 +1196,10 @@ int eb200_last_timing(eb200_timing* out) {
     Ctx& c = *t_pending;
     std::lock_guard<std::mutex> lk(c.mu);
     t_timing = eb200_timing{};
-    if (cudaEventElapsedTime(&t_timing.kernel_ms, c.ev[1], c.ev[2]) != cudaSuccess) return EB200_ERR_CUDA;
-    if (cudaEventElapsedTime(&t_timing.main_kernel_ms, c.ev[4], c.ev[5]) != cudaSuccess) return EB200_ERR_CUDA;
+    if (cudaEventElapsedTime(&t_timing.kernel_ms, c.ev[EV_INPUTS_RESIDENT], c.ev[EV_KERNELS_DONE]) != cudaSuccess)
+      return EB200_ERR_CUDA;
+    if (cudaEventElapsedTime(&t_timing.main_kernel_ms, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]) != cudaSuccess)
+      return EB200_ERR_CUDA;
     t_timing.launches = t_pending_launches;
     t_pending = nullptr;
   }
@@ -1102,23 +1218,10 @@ int eb200_ecdsa_verify_batch_dev(int curve, size_t n, const uint8_t* d_e, const 
   if (!curve_ok(curve) || !fmt_ok(pub_fmt)) return EB200_ERR_UNSUPPORTED;
   if (n == 0) return eb200_device_count() ? EB200_OK : EB200_ERR_NOT_INIT;
   if (!d_e || !d_r || !d_s || !d_pub || !d_status || !d_workspace) return EB200_ERR_ARG;
-  Ctx* cp = ctx_of(d_status);
-  if (!cp) return EB200_ERR_NOT_INIT;
-  Ctx& c = *cp;
-  std::lock_guard<std::mutex> lk(c.mu);
-  CK(cudaSetDevice(c.device));
-  int rc = ensure_table(c, curve);
-  if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;   // NULL is the CUDA default stream, as everywhere in CUDA
-  // events on the caller's stream: eb200_last_timing() reports them once the stream has been synchronised
-  CK(cudaEventRecord(c.ev[1], st));
-  unsigned launches = 0;
-  rc = launch_verify(c, curve, n, d_e, d_r, d_s, d_pub, pub_fmt, d_status, (uint8_t*)d_workspace, st, c.ev[4], c.ev[5], &launches);
-  if (rc) return rc;
-  CK(cudaEventRecord(c.ev[2], st));
-  t_pending = &c;
-  t_pending_launches = launches;
-  return EB200_OK;
+  return run_dev(d_status, curve, stream, [&](Ctx& c, Launch& L) {
+    return launch_verify(c, curve, n, d_e, d_r, d_s, d_pub, pub_fmt, d_status, (uint8_t*)d_workspace, L,
+                         c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
+  });
 }
 }  // extern "C"
 
@@ -1131,122 +1234,28 @@ static int verify_on(Ctx& c, int curve, size_t n, const uint8_t* e, const uint8_
   if (rc) return rc;
   const size_t len = curve_len(curve), pb = pub_item_bytes(len, pub_fmt);
   const ChunkPlan P = make_plan(n);
-  const int chunks = P.chunks;
-  const size_t per = P.max_m;
-  size_t item_in = 3 * len + pb;
-  if ((rc = grow(&c.d_in, &c.d_in_cap, align256(n * item_in) + 1024))) return rc;
+  if ((rc = grow(&c.d_in, &c.d_in_cap, align256(n * (3 * len + pb)) + 1024))) return rc;
   // two chunks in flight (alternating compute streams, so the grid tail of chunk k is filled by chunk k+1)
-  const size_t ws_slot = ws_layout(curve, per).total;
-  if ((rc = grow(&c.d_ws, &c.d_ws_cap, (chunks > 1 ? 2 : 1) * ws_slot))) return rc;
+  const size_t ws_slot = ws_layout(curve, P.max_m).total;
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, (P.chunks > 1 ? 2 : 1) * ws_slot))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
-  uint8_t* d_e = c.d_in;
-  uint8_t* d_r = d_e + n * len;
-  uint8_t* d_s = d_r + n * len;
-  uint8_t* d_pub = d_s + n * len;
-  cudaStream_t cs = c.copy_stream;
-  unsigned launches = 0;
-  CK(cudaEventRecord(c.ev[0], cs));
-  int used = 0;
-  for (int k = 0; k < chunks; k++) {
-    size_t lo = P.lo[k];
-    size_t m = P.lo[k + 1] - lo;
-    used = k + 1;
-    Seg seg[4] = {{d_e + lo * len, e + lo * len, m * len}, {d_r + lo * len, r + lo * len, m * len},
-                  {d_s + lo * len, s + lo * len, m * len}, {d_pub + lo * pb, pub + lo * pb, m * pb}};
-    if ((rc = h2d(c, seg, 4, cs))) return rc;
-    CK(cudaEventRecord(c.ev_in[k], cs));
-    cudaStream_t ks = (k & 1) ? c.stream2 : c.stream;
-    CK(cudaStreamWaitEvent(ks, c.ev_in[k], 0));
-    if ((rc = launch_verify(c, curve, m, d_e + lo * len, d_r + lo * len, d_s + lo * len, d_pub + lo * pb, pub_fmt,
-                            c.d_status + lo, c.d_ws + (size_t)(k & 1) * ws_slot, ks, c.ev_k0[k], c.ev_k1[k], &launches))) return rc;
-    CK(cudaEventRecord(c.ev_done[k], ks));
-  }
-  // results: one device->host copy per chunk, behind that chunk's kernels, on the copy stream
-  for (int k = 0; k < used; k++) {
-    size_t lo = P.lo[k];
-    size_t m = P.lo[k + 1] - lo;
-    CK(cudaStreamWaitEvent(cs, c.ev_done[k], 0));
-    CK(cudaMemcpyAsync(status + lo, c.d_status + lo, m, cudaMemcpyDeviceToHost, cs));
-  }
-  CK(cudaEventRecord(c.ev[3], cs));
-  CK(cudaStreamSynchronize(cs));
-  CK(cudaStreamSynchronize(c.stream));
-  CK(cudaStreamSynchronize(c.stream2));
-  float total = 0, t = 0;
-  cudaEventElapsedTime(&total, c.ev[0], c.ev[3]);
-  cudaEventElapsedTime(&c.timing.h2d_ms, c.ev[0], c.ev_in[used - 1]);       // all inputs resident
-  for (int k = 0; k < used; k++) {       // chunks overlap on two streams: report the span of the main kernels
-    cudaEventElapsedTime(&t, c.ev_k0[0], c.ev_k1[k]);
-    if (t > c.timing.main_kernel_ms) c.timing.main_kernel_ms = t;
-  }
-  cudaEventElapsedTime(&t, c.ev_done[used - 1], c.ev[3]);
-  c.timing.d2h_ms = t;                                                       // exposed tail copy
-  c.timing.kernel_ms = total;                                                // whole call on the GPU timeline
-  c.timing.launches = launches;
-  return EB200_OK;
-}
-
-// common tail of the single-stream calls: events ev[0..3] = start, inputs resident, kernels done, outputs home
-static int finish_timing(Ctx& c, unsigned launches, bool main_is_total) {
-  CK(cudaStreamSynchronize(c.stream));
-  cudaEventElapsedTime(&c.timing.h2d_ms, c.ev[0], c.ev[1]);
-  cudaEventElapsedTime(&c.timing.kernel_ms, c.ev[1], c.ev[2]);
-  cudaEventElapsedTime(&c.timing.d2h_ms, c.ev[2], c.ev[3]);
-  if (main_is_total) c.timing.main_kernel_ms = c.timing.kernel_ms;
-  else cudaEventElapsedTime(&c.timing.main_kernel_ms, c.ev[4], c.ev[5]);
-  c.timing.launches = launches;
-  return EB200_OK;
-}
-
-// Generic two-stream chunk pipeline for the fixed-stride calls: chunk k's inputs go up on the copy stream, its
-// kernels run on stream (k & 1) (so the grid tail of one chunk is filled by the next), its outputs come home on the
-// copy stream behind them.  in(lo, m, seg) / out(lo, m, seg) fill up to 8 segments (out: dst = host, src = device);
-// run(lo, m, stream, slot, k) launches the kernels and records ev_k0[k] / ev_k1[k] around the main one.
-template <class In, class Run, class Out>
-static int run_chunked(Ctx& c, const ChunkPlan& P, unsigned launches_per_chunk, In&& in, Run&& run, Out&& out) {
-  int rc;
-  cudaStream_t cs = c.copy_stream;
-  CK(cudaEventRecord(c.ev[0], cs));
-  int used = 0;
-  for (int k = 0; k < P.chunks; k++) {
-    size_t lo = P.lo[k];
-    size_t m = P.lo[k + 1] - lo;
-    used = k + 1;
-    Seg seg[8];
-    int cnt = in(lo, m, seg);
-    if ((rc = h2d(c, seg, cnt, cs))) return rc;
-    CK(cudaEventRecord(c.ev_in[k], cs));
-    cudaStream_t ks = (k & 1) ? c.stream2 : c.stream;
-    CK(cudaStreamWaitEvent(ks, c.ev_in[k], 0));
-    if ((rc = run(lo, m, ks, k & 1, k))) return rc;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(c.ev_done[k], ks));
-  }
-  for (int k = 0; k < used; k++) {
-    size_t lo = P.lo[k];
-    size_t m = P.lo[k + 1] - lo;
-    CK(cudaStreamWaitEvent(cs, c.ev_done[k], 0));
-    Seg seg[8];
-    int cnt = out(lo, m, seg);
-    for (int j = 0; j < cnt; j++)
-      if (seg[j].dst && seg[j].bytes) CK(cudaMemcpyAsync(seg[j].dst, seg[j].src, seg[j].bytes, cudaMemcpyDeviceToHost, cs));
-  }
-  CK(cudaEventRecord(c.ev[3], cs));
-  CK(cudaStreamSynchronize(cs));
-  CK(cudaStreamSynchronize(c.stream));
-  CK(cudaStreamSynchronize(c.stream2));
-  float total = 0, t = 0;
-  cudaEventElapsedTime(&total, c.ev[0], c.ev[3]);
-  cudaEventElapsedTime(&c.timing.h2d_ms, c.ev[0], c.ev_in[used - 1]);
-  for (int k = 0; k < used; k++) {
-    cudaEventElapsedTime(&t, c.ev_k0[0], c.ev_k1[k]);
-    if (t > c.timing.main_kernel_ms) c.timing.main_kernel_ms = t;
-  }
-  cudaEventElapsedTime(&t, c.ev_done[used - 1], c.ev[3]);
-  c.timing.d2h_ms = t;
-  c.timing.kernel_ms = total;
-  c.timing.launches = launches_per_chunk * (unsigned)used;
-  return EB200_OK;
+  uint8_t *d_e = c.d_in, *d_r = d_e + n * len, *d_s = d_r + n * len, *d_pub = d_s + n * len;
+  return run_chunked(c, P,
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {d_e + lo * len, e + lo * len, m * len};
+      seg[1] = {d_r + lo * len, r + lo * len, m * len};
+      seg[2] = {d_s + lo * len, s + lo * len, m * len};
+      seg[3] = {d_pub + lo * pb, pub + lo * pb, m * pb};
+      return 4;
+    },
+    [&](size_t lo, size_t m, Launch& L, int slot, int k) {
+      return launch_verify(c, curve, m, d_e + lo * len, d_r + lo * len, d_s + lo * len, d_pub + lo * pb, pub_fmt,
+                           c.d_status + lo, c.d_ws + (size_t)slot * ws_slot, L, c.ev_k0[k], c.ev_k1[k]);
+    },
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {status + lo, c.d_status + lo, m};
+      return 1;
+    });
 }
 
 // DER-encoded signatures, parsed on the GPU (variable length: concatenated bytes + offsets; sig_off points at
@@ -1267,19 +1276,12 @@ static int verify_der_on(Ctx& c, int curve, size_t n, const uint8_t* e, const ui
   uint8_t* d_s = d_r + n * len;
   uint8_t* d_pub = d_s + n * len;
   uint8_t* d_sig = d_pub + align256(n * pb);
-  cudaStream_t st = c.stream;
-  unsigned launches = 0;
-  CK(cudaEventRecord(c.ev[0], st));
-  Seg seg[4] = {{d_off, sig_off, (n + 1) * 8}, {d_e, e, n * len}, {d_pub, pub, n * pb}, {d_sig, sigs + sig_off[0], sig_bytes}};
-  if ((rc = h2d(c, seg, 4, st))) return rc;
-  CK(cudaEventRecord(c.ev[1], st));
-  // offsets are used relative to sig_off[0] on the device
-  if ((rc = launch_verify(c, curve, n, d_e, d_r, d_s, d_pub, pub_fmt, c.d_status, c.d_ws, st, c.ev[4], c.ev[5], &launches,
-                          d_sig - sig_off[0], d_off))) return rc;
-  CK(cudaEventRecord(c.ev[2], st));
-  CK(cudaMemcpyAsync(status, c.d_status, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaEventRecord(c.ev[3], st));
-  return finish_timing(c, launches, false);
+  return run_single(c, {{d_off, sig_off, (n + 1) * 8}, {d_e, e, n * len}, {d_pub, pub, n * pb}, {d_sig, sigs + sig_off[0], sig_bytes}},
+    [&](Launch& L) {     // offsets are used relative to sig_off[0] on the device
+      return launch_verify(c, curve, n, d_e, d_r, d_s, d_pub, pub_fmt, c.d_status, c.d_ws, L, c.ev[EV_MAIN_BEGIN],
+                           c.ev[EV_MAIN_END], d_sig - sig_off[0], d_off);
+    },
+    {{status, c.d_status, n}}, {}, false);
 }
 
 extern "C" {
@@ -1313,83 +1315,43 @@ int eb200_ecdsa_verify_batch_der(int curve, size_t n, const uint8_t* e, const ui
 // ---- ECDSA public-key recovery ------------------------------------------------------------
 }  // extern "C"
 
-template <class C>
-static int sw_recover_launch(Ctx& c, int curve, size_t n, const uint8_t* d_e, const uint8_t* d_r, const uint8_t* d_s, const uint8_t* d_id,
-                             uint8_t* d_out, const WsLayout& L, cudaStream_t st) {
-  unsigned nb = (unsigned)((n + 127) / 128);
-  sw_prep_recover_kernel<C><<<nb, 128, 0, st>>>(n, d_e, d_r, d_s, (u32*)(c.d_ws + L.ws));
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(c.ev[4], st));
-  sw_recover_kernel<C><<<nb, 128, 0, st>>>(n, d_r, d_id, (u32*)(c.d_ws + L.ws), c.gtab[curve], (u32*)(c.d_ws + L.qtab), d_out, c.d_status);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(c.ev[5], st));
-  return EB200_OK;
-}
-
 static int recover_on(Ctx& c, int curve, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
                       const uint8_t* recid, uint8_t* out_xy, uint8_t* status) {
   int rc = ensure_table(c, curve);
   if (rc) return rc;
   const size_t len = curve_len(curve);
-  WsLayout L = ws_layout(curve, n);
+  const WsLayout W = ws_layout(curve, n);
   if ((rc = grow(&c.d_in, &c.d_in_cap, n * (5 * len + 1) + 256))) return rc;
-  if ((rc = grow(&c.d_ws, &c.d_ws_cap, L.total))) return rc;
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, W.total))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
   uint8_t *d_e = c.d_in, *d_r = d_e + len * n, *d_s = d_r + len * n, *d_out = d_s + len * n, *d_id = d_out + 2 * len * n;
-  cudaStream_t st = c.stream;
-  CK(cudaEventRecord(c.ev[0], st));
-  Seg seg[4] = {{d_e, e, len * n}, {d_r, r, len * n}, {d_s, s, len * n}, {d_id, recid, n}};
-  if ((rc = h2d(c, seg, 4, st))) return rc;
-  CK(cudaEventRecord(c.ev[1], st));
-  if (curve == EB200_CURVE_SECP256K1) {
-    size_t T = (n + PREP_BATCH - 1) / PREP_BATCH;
-    k256_prep_recover_kernel<<<(unsigned)((T + 127) / 128), 128, 0, st>>>(n, d_e, d_r, d_s, (u32*)(c.d_ws + L.ws), (u32*)(c.d_ws + L.scratch));
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(c.ev[4], st));
-    k256_recover_kernel<<<(unsigned)((n + EB_VERIFY_BLOCK - 1) / EB_VERIFY_BLOCK), EB_VERIFY_BLOCK, 0, st>>>(
-        n, d_r, d_id, (u32*)(c.d_ws + L.ws), c.gtab[curve], (u32*)(c.d_ws + L.qtab), d_out, c.d_status);
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(c.ev[5], st));
-  } else {
-#define EB_REC(C) sw_recover_launch<C>(c, curve, n, d_e, d_r, d_s, d_id, d_out, L, st)
-    rc = SW_DISPATCH(curve, EB_REC);
-#undef EB_REC
-    if (rc) return rc;
-  }
-  CK(cudaEventRecord(c.ev[2], st));
-  CK(cudaMemcpyAsync(out_xy, d_out, 2 * len * n, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(status, c.d_status, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaEventRecord(c.ev[3], st));
-  return finish_timing(c, 2, false);
+  u32 *ws = (u32*)(c.d_ws + W.ws), *qtab = (u32*)(c.d_ws + W.qtab);
+  return run_single(c, {{d_e, e, len * n}, {d_r, r, len * n}, {d_s, s, len * n}, {d_id, recid, n}},
+    [&](Launch& L) {
+      return with_curve(curve, [&](auto cv) {
+        typedef decltype(cv) T;
+        if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;     // eb200_ecdsa_recover_batch refuses it first
+        else {
+          if constexpr (is_k256<T>) {
+            L(k256_prep_recover_kernel, batch_blocks(n, PREP_BATCH), 128, n, d_e, d_r, d_s, ws, (u32*)(c.d_ws + W.scratch));
+            CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
+            L(k256_recover_kernel, (unsigned)((n + EB_VERIFY_BLOCK - 1) / EB_VERIFY_BLOCK), EB_VERIFY_BLOCK, n, d_r, d_id, ws,
+              c.gtab[curve], qtab, d_out, c.d_status);
+          } else {
+            L(sw_prep_recover_kernel<typename T::C>, blocks128(n), 128, n, d_e, d_r, d_s, ws);
+            CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
+            L(sw_recover_kernel<typename T::C>, blocks128(n), 128, n, d_r, d_id, ws, c.gtab[curve], qtab, d_out, c.d_status);
+          }
+          CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
+          return EB200_OK;
+        }
+      });
+    },
+    {{out_xy, d_out, 2 * len * n}, {status, c.d_status, n}}, {}, false);
 }
 
 // ---- Point.mul / Point.mulAdd batches ---------------------------------------------------------------
 // k1 == NULL: k2*P;  pts == NULL: k2*G;  both given: k1*G + k2*P.
-template <class C>
-static int sw_mul_add_launch(Ctx& c, int curve, size_t n, const uint8_t* d_k1, const uint8_t* d_k2, const uint8_t* d_pts,
-                             uint8_t* d_out, const WsLayout& L, cudaStream_t st, unsigned* launches, bool derive) {
-  unsigned nb = (unsigned)((n + 127) / 128);
-  if (!d_pts) {
-    CK(cudaEventRecord(c.ev[4], st));
-    sw_mul_g_kernel<C><<<nb, 128, 0, st>>>(n, d_k2, c.gtab[curve], d_out, c.d_status);
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(c.ev[5], st));
-    *launches = 1;
-    return EB200_OK;
-  }
-  sw_prep_scalars_kernel<C><<<nb, 128, 0, st>>>(n, d_k1, d_k2, (u32*)(c.d_ws + L.ws));
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(c.ev[4], st));
-  sw_mul_add_kernel<C><<<nb, 128, 0, st>>>(n, d_pts, (u32*)(c.d_ws + L.ws), c.gtab[curve], (u32*)(c.d_ws + L.qtab), d_out, c.d_status);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(c.ev[5], st));
-  if (derive) status_map_kernel<<<nb, 128, 0, st>>>(n, c.d_status, ST_NEEDS_HOST, ST_THROW_NOT_VALIDATED);
-  else sw_mul_add_replay_kernel<C><<<nb, 128, 0, st>>>(n, d_k1, d_k2, d_pts, c.sw_replay_tab[curve], d_out, c.d_status);
-  CK(cudaGetLastError());
-  *launches = 3;
-  return EB200_OK;
-}
-
 // derive: KeyPair.derive (ec/key.js:102-107) -- an off-curve point is the reference's
 // 'public point not validated' throw instead of a replayed multiplication, and only x is returned.
 static int mul_add_on(Ctx& c, int curve, size_t n, const uint8_t* k1, const uint8_t* k2, const uint8_t* pts,
@@ -1397,58 +1359,50 @@ static int mul_add_on(Ctx& c, int curve, size_t n, const uint8_t* k1, const uint
   int rc = ensure_table(c, curve);
   if (rc) return rc;
   const size_t len = curve_len(curve);
-  WsLayout L = ws_layout(curve, n);
+  const WsLayout W = ws_layout(curve, n);
   if ((rc = grow(&c.d_in, &c.d_in_cap, n * 6 * len + 256))) return rc;
-  if ((rc = grow(&c.d_ws, &c.d_ws_cap, L.total))) return rc;
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, W.total))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
   uint8_t *d_k1 = c.d_in, *d_k2 = d_k1 + len * n, *d_pts = d_k2 + len * n, *d_out = d_pts + 2 * len * n;
-  cudaStream_t st = c.stream;
-  unsigned nb = (unsigned)((n + 127) / 128), launches = 0;
-  CK(cudaEventRecord(c.ev[0], st));
-  Seg seg[3] = {{d_k1, k1, k1 ? len * n : 0}, {d_k2, k2, len * n}, {d_pts, pts, pts ? 2 * len * n : 0}};
-  if ((rc = h2d(c, seg, 3, st))) return rc;
-  CK(cudaEventRecord(c.ev[1], st));
-  if (curve == EB200_CURVE_ED25519) {
-    CK(cudaEventRecord(c.ev[4], st));
-    ed_ec_mul_add_kernel<<<nb, 128, 0, st>>>(n, k1 ? d_k1 : nullptr, d_k2, pts ? d_pts : nullptr, derive ? 1u : 0u, c.gtab[curve],
-                                             (u32*)(c.d_ws + L.qtab), d_out, c.d_status);
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(c.ev[5], st));
-    launches = 1;
-  } else if (curve != EB200_CURVE_SECP256K1) {
-#define EB_MA(C) sw_mul_add_launch<C>(c, curve, n, k1 ? d_k1 : nullptr, d_k2, pts ? d_pts : nullptr, d_out, L, st, &launches, derive)
-    if ((rc = SW_DISPATCH(curve, EB_MA))) return rc;
-#undef EB_MA
-  } else if (!pts) {
-    CK(cudaEventRecord(c.ev[4], st));
-    k256_mul_g_kernel<<<nb, 128, 0, st>>>(n, d_k2, c.gtab[curve], d_out, c.d_status);
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(c.ev[5], st));
-    launches = 1;
-  } else {
-    k256_prep_scalars_kernel<<<nb, 128, 0, st>>>(n, k1 ? d_k1 : nullptr, d_k2, (u32*)(c.d_ws + L.ws));
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(c.ev[4], st));
-    k256_mul_add_kernel<<<(unsigned)((n + EB_VERIFY_BLOCK - 1) / EB_VERIFY_BLOCK), EB_VERIFY_BLOCK, 0, st>>>(
-        n, d_pts, (u32*)(c.d_ws + L.ws), c.gtab[curve], (u32*)(c.d_ws + L.qtab), d_out, c.d_status);
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(c.ev[5], st));
-    if (derive) status_map_kernel<<<nb, 128, 0, st>>>(n, c.d_status, ST_NEEDS_HOST, ST_THROW_NOT_VALIDATED);
-    else k256_mul_add_replay_kernel<<<nb, 128, 0, st>>>(n, k1 ? d_k1 : nullptr, d_k2, d_pts, c.replay_tab, d_out, c.d_status);
-    CK(cudaGetLastError());
-    launches = 3;
-  }
-  CK(cudaEventRecord(c.ev[2], st));
-  if (derive) {
-    CK(cudaMemcpy2DAsync(out_xy, len, d_out, 2 * len, len, n, cudaMemcpyDeviceToHost, st));   // x only
-    // the scalars of an ECDH call are private keys: do not leave them in the shared staging buffer
-    CK(cudaMemsetAsync(d_k2, 0, len * n, st));
-  } else {
-    CK(cudaMemcpyAsync(out_xy, d_out, 2 * len * n, cudaMemcpyDeviceToHost, st));
-  }
-  CK(cudaMemcpyAsync(status, c.d_status, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaEventRecord(c.ev[3], st));
-  return finish_timing(c, launches, false);
+  const uint8_t* dk1 = k1 ? d_k1 : nullptr;
+  u32 *ws = (u32*)(c.d_ws + W.ws), *qtab = (u32*)(c.d_ws + W.qtab);
+  const unsigned nb = blocks128(n);
+  return run_single(c, {{d_k1, k1, k1 ? len * n : 0}, {d_k2, k2, len * n}, {d_pts, pts, pts ? 2 * len * n : 0}},
+    [&](Launch& L) {
+      return with_curve(curve, [&](auto cv) {
+        typedef decltype(cv) T;
+        const u32* gt = c.gtab[curve];
+        if constexpr (is_ed25519<T>) {
+          CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
+          L(ed_ec_mul_add_kernel, nb, 128, n, dk1, d_k2, pts ? d_pts : nullptr, derive ? 1u : 0u, gt, qtab, d_out, c.d_status);
+          CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
+        } else if (!pts) {
+          CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
+          if constexpr (is_k256<T>) L(k256_mul_g_kernel, nb, 128, n, d_k2, gt, d_out, c.d_status);
+          else L(sw_mul_g_kernel<typename T::C>, nb, 128, n, d_k2, gt, d_out, c.d_status);
+          CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
+        } else {
+          if constexpr (is_k256<T>) {
+            L(k256_prep_scalars_kernel, nb, 128, n, dk1, d_k2, ws);
+            CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
+            L(k256_mul_add_kernel, (unsigned)((n + EB_VERIFY_BLOCK - 1) / EB_VERIFY_BLOCK), EB_VERIFY_BLOCK, n, d_pts, ws, gt,
+              qtab, d_out, c.d_status);
+          } else {
+            L(sw_prep_scalars_kernel<typename T::C>, nb, 128, n, dk1, d_k2, ws);
+            CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
+            L(sw_mul_add_kernel<typename T::C>, nb, 128, n, d_pts, ws, gt, qtab, d_out, c.d_status);
+          }
+          CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
+          if (derive) L(status_map_kernel, nb, 128, n, c.d_status, (uint8_t)ST_NEEDS_HOST, (uint8_t)ST_THROW_NOT_VALIDATED);
+          else if constexpr (is_k256<T>) L(k256_mul_add_replay_kernel, nb, 128, n, dk1, d_k2, d_pts, c.replay_tab, d_out, c.d_status);
+          else L(sw_mul_add_replay_kernel<typename T::C>, nb, 128, n, dk1, d_k2, d_pts, c.sw_replay_tab[curve], d_out, c.d_status);
+        }
+        return EB200_OK;
+      });
+    },
+    // derive: x only; its scalars are private keys, which do not stay in the shared staging buffer
+    {{out_xy, d_out, derive ? len : 2 * len * n, derive ? n : 1, 2 * len}, {status, c.d_status, n}},
+    {{d_k2, derive ? len * n : 0}}, false);
 }
 
 static int mul_add_common(int curve, size_t n, const uint8_t* k1, const uint8_t* k2, const uint8_t* pts,
@@ -1467,27 +1421,6 @@ static int mul_add_common(int curve, size_t n, const uint8_t* k1, const uint8_t*
 // ---- ECDSA sign (RFC 6979 nonces on the GPU) ---------------------------------------------------------
 // mode: kgiven != NULL -> the caller's nonces, one attempt (items the reference would `continue` on come back as
 // EB200_ST_RETRY); pers != NULL -> the literal loop on the byte-stream DRBG; neither -> RFC 6979 fast pipeline.
-template <class SG>
-static int sw_sign_launch(Ctx& c, int curve, size_t n, const uint8_t* d_e, const uint8_t* d_k, u32 canonical, u32* d_sws, u32* d_scr,
-                          uint8_t* d_r, uint8_t* d_s, uint8_t* d_id, cudaStream_t st, const uint8_t* d_kgiven,
-                          const uint8_t* d_pers, u32 np) {
-  unsigned nb = (unsigned)((n + 127) / 128);
-  if (d_pers) {
-    sw_sign_pers_kernel<SG><<<nb, 128, 0, st>>>(n, d_e, d_k, d_pers, np, canonical, c.gtab[curve], d_r, d_s, d_id, c.d_status);
-    CK(cudaGetLastError());
-    return EB200_OK;
-  }
-  size_t T = (n + SG::BATCH - 1) / SG::BATCH;
-  sw_sign_nonce_kernel<SG><<<nb, 128, 0, st>>>(n, d_e, d_k, c.gtab[curve], d_sws, c.d_status, d_kgiven);
-  CK(cudaGetLastError());
-  sw_sign_finish_kernel<SG><<<(unsigned)((T + 127) / 128), 128, 0, st>>>(n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, c.d_status);
-  CK(cudaGetLastError());
-  if (d_kgiven) status_map_kernel<<<nb, 128, 0, st>>>(n, c.d_status, ST_NEEDS_HOST, EB200_ST_RETRY);
-  else sw_sign_slow_kernel<SG><<<nb, 128, 0, st>>>(n, d_e, d_k, canonical, c.gtab[curve], d_r, d_s, d_id, c.d_status);
-  CK(cudaGetLastError());
-  return EB200_OK;
-}
-
 static int sign_on(Ctx& c, int curve, size_t n, const uint8_t* e, const uint8_t* priv, uint32_t flags,
                    uint8_t* out_r, uint8_t* out_s, uint8_t* out_recid, uint8_t* status,
                    const uint8_t* kgiven = nullptr, const uint8_t* pers = nullptr, size_t np = 0) {
@@ -1503,55 +1436,40 @@ static int sign_on(Ctx& c, int curve, size_t n, const uint8_t* e, const uint8_t*
   uint8_t* d_pers = (uint8_t*)(((uintptr_t)(d_id + n) + 255) & ~(uintptr_t)255);
   u32 *d_sws = (u32*)c.d_ws, *d_scr = (u32*)(c.d_ws + ws_bytes);
   const u32 canonical = flags & EB200_SIGN_CANONICAL;
-  cudaStream_t st = c.stream;
-  CK(cudaEventRecord(c.ev[0], st));
-  Seg seg[4] = {{d_e, e, len * n}, {d_k, priv, len * n}, {d_kg, kgiven, kgiven ? len * n : 0}, {d_pers, pers, pers ? np : 0}};
-  if ((rc = h2d(c, seg, 4, st))) return rc;
-  CK(cudaEventRecord(c.ev[1], st));
   const uint8_t* kg = kgiven ? d_kg : nullptr;
   const uint8_t* pp = pers ? d_pers : nullptr;
-  if (curve == EB200_CURVE_ED25519) {
-    static const uint8_t* none = nullptr;
-    (void)none;
-    ed_ec_sign_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, d_e, d_k, kg, pp, (u32)np, canonical, c.gtab[curve], d_r, d_s, d_id, c.d_status);
-    CK(cudaGetLastError());
-  } else if (curve == EB200_CURVE_P256) {
-    if ((rc = sw_sign_launch<SWSign<P256, Sha256W>>(c, curve, n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, st, kg, pp, (u32)np))) return rc;
-  } else if (curve == EB200_CURVE_P384) {
-    if ((rc = sw_sign_launch<SWSign<P384, Sha384W>>(c, curve, n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, st, kg, pp, (u32)np))) return rc;
-  } else if (curve == EB200_CURVE_P521) {     // curves.js:124, 50, 65: sha512, sha256, sha256
-    if ((rc = sw_sign_launch<SWSign<P521, Sha512W>>(c, curve, n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, st, kg, pp, (u32)np))) return rc;
-  } else if (curve == EB200_CURVE_P192) {
-    if ((rc = sw_sign_launch<SWSign<P192, Sha256W>>(c, curve, n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, st, kg, pp, (u32)np))) return rc;
-  } else if (curve == EB200_CURVE_P224) {
-    if ((rc = sw_sign_launch<SWSign<P224, Sha256W>>(c, curve, n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, st, kg, pp, (u32)np))) return rc;
-  } else {
-    unsigned nb = (unsigned)((n + 127) / 128);
-    size_t T = (n + PREP_BATCH - 1) / PREP_BATCH;
-    if (pp) {
-      k256_sign_pers_kernel<<<nb, 128, 0, st>>>(n, d_e, d_k, pp, (u32)np, canonical, c.gtab[curve], d_r, d_s, d_id, c.d_status);
-      CK(cudaGetLastError());
-    } else {
-      k256_sign_nonce_kernel<<<nb, 128, 0, st>>>(n, d_e, d_k, c.gtab[curve], d_sws, c.d_status, kg);
-      CK(cudaGetLastError());
-      k256_sign_finish_kernel<<<(unsigned)((T + 127) / 128), 128, 0, st>>>(n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, c.d_status);
-      CK(cudaGetLastError());
-      if (kg) status_map_kernel<<<nb, 128, 0, st>>>(n, c.d_status, ST_NEEDS_HOST, EB200_ST_RETRY);
-      else k256_sign_slow_kernel<<<nb, 128, 0, st>>>(n, d_e, d_k, canonical, c.gtab[curve], d_r, d_s, d_id, c.d_status);
-      CK(cudaGetLastError());
-    }
-  }
-  CK(cudaEventRecord(c.ev[2], st));
-  CK(cudaMemcpyAsync(out_r, d_r, len * n, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(out_s, d_s, len * n, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(out_recid, d_id, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(status, c.d_status, n, cudaMemcpyDeviceToHost, st));
-  // private keys, nonces k and k*G live in buffers that later calls reuse: wipe them before returning
-  CK(cudaMemsetAsync(d_k, 0, len * n, st));
-  if (kgiven) CK(cudaMemsetAsync(d_kg, 0, len * n, st));
-  CK(cudaMemsetAsync(c.d_ws, 0, ws_bytes + scr_bytes, st));
-  CK(cudaEventRecord(c.ev[3], st));
-  return finish_timing(c, pp ? 1 : 3, true);
+  const unsigned nb = blocks128(n);
+  return run_single(c, {{d_e, e, len * n}, {d_k, priv, len * n}, {d_kg, kgiven, kgiven ? len * n : 0}, {d_pers, pers, pers ? np : 0}},
+    [&](Launch& L) {
+      return with_curve(curve, [&](auto cv) {
+        typedef decltype(cv) T;
+        const u32* gt = c.gtab[curve];
+        if constexpr (is_ed25519<T>) {
+          L(ed_ec_sign_kernel, nb, 128, n, d_e, d_k, kg, pp, (u32)np, canonical, gt, d_r, d_s, d_id, c.d_status);
+        } else if constexpr (is_k256<T>) {
+          if (pp) L(k256_sign_pers_kernel, nb, 128, n, d_e, d_k, pp, (u32)np, canonical, gt, d_r, d_s, d_id, c.d_status);
+          else {
+            L(k256_sign_nonce_kernel, nb, 128, n, d_e, d_k, gt, d_sws, c.d_status, kg);
+            L(k256_sign_finish_kernel, batch_blocks(n, PREP_BATCH), 128, n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, c.d_status);
+            if (kg) L(status_map_kernel, nb, 128, n, c.d_status, (uint8_t)ST_NEEDS_HOST, (uint8_t)EB200_ST_RETRY);
+            else L(k256_sign_slow_kernel, nb, 128, n, d_e, d_k, canonical, gt, d_r, d_s, d_id, c.d_status);
+          }
+        } else {
+          typedef typename T::SG SG;
+          if (pp) L(sw_sign_pers_kernel<SG>, nb, 128, n, d_e, d_k, pp, (u32)np, canonical, gt, d_r, d_s, d_id, c.d_status);
+          else {
+            L(sw_sign_nonce_kernel<SG>, nb, 128, n, d_e, d_k, gt, d_sws, c.d_status, kg);
+            L(sw_sign_finish_kernel<SG>, batch_blocks(n, SG::BATCH), 128, n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, c.d_status);
+            if (kg) L(status_map_kernel, nb, 128, n, c.d_status, (uint8_t)ST_NEEDS_HOST, (uint8_t)EB200_ST_RETRY);
+            else L(sw_sign_slow_kernel<SG>, nb, 128, n, d_e, d_k, canonical, gt, d_r, d_s, d_id, c.d_status);
+          }
+        }
+        return EB200_OK;
+      });
+    },
+    {{out_r, d_r, len * n}, {out_s, d_s, len * n}, {out_recid, d_id, n}, {status, c.d_status, n}},
+    // private keys, nonces k and k*G live in buffers that later calls reuse: wipe them before returning
+    {{d_k, len * n}, {d_kg, kgiven ? len * n : 0}, {c.d_ws, ws_bytes + scr_bytes}}, true);
 }
 
 // EC.genKeyPair({entropy, pers}) (ec/index.js:55-79): private keys from HMAC-DRBG(entropy_i, nonce = n, pers), then
@@ -1567,39 +1485,26 @@ static int keygen_on(Ctx& c, int curve, size_t n, const uint8_t* entropy, size_t
   uint8_t* d_pers = d_ent + align256(n * ne);
   uint8_t* d_priv = d_pers + align256(np + 1);
   uint8_t* d_pub = d_priv + len * n;
-  cudaStream_t st = c.stream;
-  unsigned nb = (unsigned)((n + 127) / 128);
-  CK(cudaEventRecord(c.ev[0], st));
-  Seg seg[2] = {{d_ent, entropy, n * ne}, {d_pers, pers, pers ? np : 0}};
-  if ((rc = h2d(c, seg, 2, st))) return rc;
-  CK(cudaEventRecord(c.ev[1], st));
+  const unsigned nb = blocks128(n);
   const uint8_t* pp = pers ? d_pers : nullptr;
-  switch (curve) {
-    case EB200_CURVE_ED25519: ed_ec_keygen_kernel<<<nb, 128, 0, st>>>(n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status); break;
-    case EB200_CURVE_SECP256K1: k256_keygen_kernel<<<nb, 128, 0, st>>>(n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status); break;
-    case EB200_CURVE_P256: sw_keygen_kernel<SWSign<P256, Sha256W>><<<nb, 128, 0, st>>>(n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status); break;
-    case EB200_CURVE_P384: sw_keygen_kernel<SWSign<P384, Sha384W>><<<nb, 128, 0, st>>>(n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status); break;
-    case EB200_CURVE_P521: sw_keygen_kernel<SWSign<P521, Sha512W>><<<nb, 128, 0, st>>>(n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status); break;
-    case EB200_CURVE_P192: sw_keygen_kernel<SWSign<P192, Sha256W>><<<nb, 128, 0, st>>>(n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status); break;
-    default: sw_keygen_kernel<SWSign<P224, Sha256W>><<<nb, 128, 0, st>>>(n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status); break;
-  }
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(status, c.d_status, n, cudaMemcpyDeviceToHost, st));      // the keygen verdicts (the mul below reuses d_status)
-  if (curve == EB200_CURVE_SECP256K1) k256_mul_g_kernel<<<nb, 128, 0, st>>>(n, d_priv, c.gtab[curve], d_pub, c.d_status);
-  else if (curve == EB200_CURVE_ED25519) ed_ec_mul_add_kernel<<<nb, 128, 0, st>>>(n, nullptr, d_priv, nullptr, 0u, c.gtab[curve], nullptr, d_pub, c.d_status);
-  else {
-#define EB_KG(C) (sw_mul_g_kernel<C><<<nb, 128, 0, st>>>(n, d_priv, c.gtab[curve], d_pub, c.d_status), 0)
-    (void)SW_DISPATCH(curve, EB_KG);
-#undef EB_KG
-  }
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(c.ev[2], st));
-  CK(cudaMemcpyAsync(out_priv, d_priv, len * n, cudaMemcpyDeviceToHost, st));
-  if (out_pub) CK(cudaMemcpyAsync(out_pub, d_pub, 2 * len * n, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemsetAsync(d_ent, 0, n * ne, st));
-  CK(cudaMemsetAsync(d_priv, 0, len * n, st));
-  CK(cudaEventRecord(c.ev[3], st));
-  return finish_timing(c, 2, true);
+  return run_single(c, {{d_ent, entropy, n * ne}, {d_pers, pers, pers ? np : 0}},
+    [&](Launch& L) {
+      return with_curve(curve, [&](auto cv) {
+        typedef decltype(cv) T;
+        const u32* gt = c.gtab[curve];
+        if constexpr (is_k256<T>) L(k256_keygen_kernel, nb, 128, n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status);
+        else if constexpr (is_ed25519<T>) L(ed_ec_keygen_kernel, nb, 128, n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status);
+        else L(sw_keygen_kernel<typename T::SG>, nb, 128, n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status);
+        if (L.rc) return L.rc;
+        // the keygen verdicts (the mul below reuses d_status)
+        CK(cudaMemcpyAsync(status, c.d_status, n, cudaMemcpyDeviceToHost, L.st));
+        if constexpr (is_k256<T>) L(k256_mul_g_kernel, nb, 128, n, d_priv, gt, d_pub, c.d_status);
+        else if constexpr (is_ed25519<T>) L(ed_ec_mul_add_kernel, nb, 128, n, nullptr, d_priv, nullptr, 0u, gt, nullptr, d_pub, c.d_status);
+        else L(sw_mul_g_kernel<typename T::C>, nb, 128, n, d_priv, gt, d_pub, c.d_status);
+        return EB200_OK;
+      });
+    },
+    {{out_priv, d_priv, len * n}, {out_pub, d_pub, 2 * len * n}}, {{d_ent, n * ne}, {d_priv, len * n}}, true);
 }
 
 extern "C" {
@@ -1697,24 +1602,12 @@ int eb200_eddsa_verify_batch_dev(size_t n, const uint8_t* d_R, const uint8_t* d_
                                  const uint8_t* d_h, uint8_t* d_status, void* d_workspace, void* stream) {
   if (n == 0) return eb200_device_count() ? EB200_OK : EB200_ERR_NOT_INIT;
   if (!d_R || !d_S || !d_A || !d_h || !d_status || !d_workspace) return EB200_ERR_ARG;
-  Ctx* cp = ctx_of(d_status);
-  if (!cp) return EB200_ERR_NOT_INIT;
-  Ctx& c = *cp;
-  std::lock_guard<std::mutex> lk(c.mu);
-  CK(cudaSetDevice(c.device));
-  int rc = ensure_table(c, EB200_CURVE_ED25519);
-  if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  CK(cudaEventRecord(c.ev[1], st));
-  CK(cudaEventRecord(c.ev[4], st));
-  ed25519_verify_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, d_R, d_S, d_A, d_h, c.gtab[EB200_CURVE_ED25519],
-                                                                   (u32*)d_workspace, d_status);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(c.ev[5], st));
-  CK(cudaEventRecord(c.ev[2], st));
-  t_pending = &c;
-  t_pending_launches = 1;
-  return EB200_OK;
+  return run_dev(d_status, EB200_CURVE_ED25519, stream, [&](Ctx& c, Launch& L) {
+    CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
+    L(ed25519_verify_kernel, blocks128(n), 128, n, d_R, d_S, d_A, d_h, c.gtab[EB200_CURVE_ED25519], (u32*)d_workspace, d_status);
+    CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
+    return EB200_OK;
+  });
 }
 }  // extern "C"
 
@@ -1737,7 +1630,7 @@ static int eddsa_on(Ctx& c, size_t n, const uint8_t* R, const uint8_t* S, const 
   uint64_t* doff = (uint64_t*)(c.d_in + base);
   uint8_t* dm = c.d_in + base + align256(off_bytes);
   const u32* gt = c.gtab[EB200_CURVE_ED25519];
-  return run_chunked(c, P, h ? 1u : 2u,
+  return run_chunked(c, P,
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {dR + 32 * lo, R + 32 * lo, 32 * m};
       seg[1] = {dS + 32 * lo, S + 32 * lo, 32 * m};
@@ -1747,13 +1640,13 @@ static int eddsa_on(Ctx& c, size_t n, const uint8_t* R, const uint8_t* S, const 
       seg[4] = {dm + (msg_off[lo] - msg_off[0]), msgs + msg_off[lo], (size_t)(msg_off[lo + m] - msg_off[lo])};
       return 5;
     },
-    [&](size_t lo, size_t m, cudaStream_t ks, int slot, int k) {
-      unsigned nb = (unsigned)((m + 127) / 128);
-      if (!h) ed25519_hash_kernel<<<nb, 128, 0, ks>>>(m, dR + 32 * lo, dA + 32 * lo, dm - msg_off[0], doff + lo, dh + 32 * lo);
-      CK(cudaEventRecord(c.ev_k0[k], ks));
-      ed25519_verify_kernel<<<nb, 128, 0, ks>>>(m, dR + 32 * lo, dS + 32 * lo, dA + 32 * lo, dh + 32 * lo, gt,
-                                                (u32*)(c.d_ws + (size_t)slot * ws_slot), c.d_status + lo);
-      CK(cudaEventRecord(c.ev_k1[k], ks));
+    [&](size_t lo, size_t m, Launch& L, int slot, int k) {
+      const unsigned nb = blocks128(m);
+      if (!h) L(ed25519_hash_kernel, nb, 128, m, dR + 32 * lo, dA + 32 * lo, dm - msg_off[0], doff + lo, dh + 32 * lo);
+      CK(cudaEventRecord(c.ev_k0[k], L.st));
+      L(ed25519_verify_kernel, nb, 128, m, dR + 32 * lo, dS + 32 * lo, dA + 32 * lo, dh + 32 * lo, gt,
+        (u32*)(c.d_ws + (size_t)slot * ws_slot), c.d_status + lo);
+      CK(cudaEventRecord(c.ev_k1[k], L.st));
       return EB200_OK;
     },
     [&](size_t lo, size_t m, Seg* seg) {
@@ -1775,20 +1668,13 @@ static int eddsa_sign_on(Ctx& c, size_t n, const uint8_t* secrets, const uint8_t
   uint8_t *dsec = c.d_in, *dsig = dsec + 32 * n, *dpub = dsig + 64 * n;
   uint64_t* doff = (uint64_t*)(c.d_in + base);
   uint8_t* dm = c.d_in + base + align256(off_bytes);
-  cudaStream_t st = c.stream;
-  CK(cudaEventRecord(c.ev[0], st));
-  Seg seg[3] = {{dsec, secrets, 32 * n}, {doff, msg_off, off_bytes}, {dm, msgs + msg_off[0], mbytes}};
-  if ((rc = h2d(c, seg, 3, st))) return rc;
-  CK(cudaEventRecord(c.ev[1], st));
-  ed25519_sign_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, dsec, dm - msg_off[0], doff, c.gtab[EB200_CURVE_ED25519], dsig, dpub, c.d_status);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(c.ev[2], st));
-  CK(cudaMemcpyAsync(sig, dsig, 64 * n, cudaMemcpyDeviceToHost, st));
-  if (pub) CK(cudaMemcpyAsync(pub, dpub, 32 * n, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(status, c.d_status, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemsetAsync(dsec, 0, 32 * n, st));             // secrets do not stay in the shared buffer
-  CK(cudaEventRecord(c.ev[3], st));
-  return finish_timing(c, 1, true);
+  return run_single(c, {{dsec, secrets, 32 * n}, {doff, msg_off, off_bytes}, {dm, msgs + msg_off[0], mbytes}},
+    [&](Launch& L) {
+      L(ed25519_sign_kernel, blocks128(n), 128, n, dsec, dm - msg_off[0], doff, c.gtab[EB200_CURVE_ED25519], dsig, dpub, c.d_status);
+      return EB200_OK;
+    },
+    {{sig, dsig, 64 * n}, {pub, dpub, 32 * n}, {status, c.d_status, n}},
+    {{dsec, 32 * n}}, true);             // secrets do not stay in the shared buffer
 }
 
 static int x25519_on(Ctx& c, size_t n, const uint8_t* priv, const uint8_t* pubx, uint8_t* out, uint8_t* status, bool validate) {
@@ -1797,19 +1683,18 @@ static int x25519_on(Ctx& c, size_t n, const uint8_t* priv, const uint8_t* pubx,
   if ((rc = grow(&c.d_in, &c.d_in_cap, n * 96))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
   uint8_t *dk = c.d_in, *dx = dk + 32 * n, *dout = dx + 32 * n;
-  return run_chunked(c, P, 1u,
+  return run_chunked(c, P,
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {dk + 32 * lo, priv + 32 * lo, 32 * m};
       seg[1] = {dx + 32 * lo, pubx + 32 * lo, 32 * m};
       return 2;
     },
-    [&](size_t lo, size_t m, cudaStream_t ks, int, int k) {
-      unsigned nb = (unsigned)((m + 127) / 128);
-      CK(cudaEventRecord(c.ev_k0[k], ks));
-      if (validate) x25519_derive_kernel<<<nb, 128, 0, ks>>>(m, dk + 32 * lo, dx + 32 * lo, dout + 32 * lo, c.d_status + lo);
-      else x25519_mul_kernel<<<nb, 128, 0, ks>>>(m, dk + 32 * lo, dx + 32 * lo, dout + 32 * lo, c.d_status + lo);
-      CK(cudaEventRecord(c.ev_k1[k], ks));
-      CK(cudaMemsetAsync(dk + 32 * lo, 0, 32 * m, ks));   // private scalars do not stay in the shared buffer
+    [&](size_t lo, size_t m, Launch& L, int, int k) {
+      CK(cudaEventRecord(c.ev_k0[k], L.st));
+      L(validate ? x25519_derive_kernel : x25519_mul_kernel, blocks128(m), 128, m, dk + 32 * lo, dx + 32 * lo, dout + 32 * lo,
+        c.d_status + lo);
+      CK(cudaEventRecord(c.ev_k1[k], L.st));
+      CK(cudaMemsetAsync(dk + 32 * lo, 0, 32 * m, L.st));   // private scalars do not stay in the shared buffer
       return EB200_OK;
     },
     [&](size_t lo, size_t m, Seg* seg) {
@@ -1864,21 +1749,12 @@ int eb200_x25519_derive_batch_dev(size_t n, const uint8_t* d_priv, const uint8_t
                                   uint8_t* d_status, void* stream) {
   if (n == 0) return eb200_device_count() ? EB200_OK : EB200_ERR_NOT_INIT;
   if (!d_priv || !d_pubx || !d_out || !d_status) return EB200_ERR_ARG;
-  Ctx* cp = ctx_of(d_status);
-  if (!cp) return EB200_ERR_NOT_INIT;
-  Ctx& c = *cp;
-  std::lock_guard<std::mutex> lk(c.mu);
-  CK(cudaSetDevice(c.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  CK(cudaEventRecord(c.ev[1], st));
-  CK(cudaEventRecord(c.ev[4], st));
-  x25519_derive_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, d_priv, d_pubx, d_out, d_status);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(c.ev[5], st));
-  CK(cudaEventRecord(c.ev[2], st));
-  t_pending = &c;
-  t_pending_launches = 1;
-  return EB200_OK;
+  return run_dev(d_status, 0, stream, [&](Ctx& c, Launch& L) {
+    CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
+    L(x25519_derive_kernel, blocks128(n), 128, n, d_priv, d_pubx, d_out, d_status);
+    CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
+    return EB200_OK;
+  });
 }
 
 int eb200_x25519_derive_batch(size_t n, const uint8_t* priv, const uint8_t* pubx, uint8_t* out, uint8_t* status) {
@@ -1967,19 +1843,13 @@ int rt_on(Ctx& c, const RtCurve<NL>& C, int op, size_t n, const uint8_t* k1, con
   if ((rc = grow(&c.d_in, &c.d_in_cap, n * (2 * klen + 3 * pl) + 1024))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
   uint8_t *dk1 = c.d_in, *dk2 = dk1 + klen * n, *dp1 = dk2 + klen * n, *dp2 = dp1 + pl * n, *dout = dp2 + pl * n;
-  cudaStream_t st = c.stream;
-  CK(cudaEventRecord(c.ev[0], st));
-  Seg seg[4] = {{dk1, k1, k1 ? klen * n : 0}, {dk2, k2, k2 ? klen * n : 0}, {dp1, p1, pl * n}, {dp2, p2, p2 ? pl * n : 0}};
-  if ((rc = h2d(c, seg, 4, st))) return rc;
-  CK(cudaEventRecord(c.ev[1], st));
-  rt_curve_kernel<NL><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(op, n, C, k1 ? dk1 : nullptr, dp1, k2 ? dk2 : nullptr, p2 ? dp2 : nullptr,
-                                                                   (u32)klen, dout, c.d_status);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(c.ev[2], st));
-  if (op != 3) CK(cudaMemcpyAsync(out, dout, pl * n, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(status, c.d_status, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaEventRecord(c.ev[3], st));
-  return finish_timing(c, 1, true);
+  return run_single(c, {{dk1, k1, k1 ? klen * n : 0}, {dk2, k2, k2 ? klen * n : 0}, {dp1, p1, pl * n}, {dp2, p2, p2 ? pl * n : 0}},
+    [&](Launch& L) {
+      L(rt_curve_kernel<NL>, blocks128(n), 128, op, n, C, k1 ? dk1 : nullptr, dp1, k2 ? dk2 : nullptr, p2 ? dp2 : nullptr,
+        (u32)klen, dout, c.d_status);
+      return EB200_OK;
+    },
+    {{op != 3 ? out : nullptr, dout, pl * n}, {status, c.d_status, n}}, {}, true);
 }
 template <int NL>
 int rt_call(const eb200_short_curve* cv, int op, size_t n, const uint8_t* k1, const uint8_t* p1, const uint8_t* k2, const uint8_t* p2,
@@ -2050,14 +1920,14 @@ int eb200_selftest_fe(int curve, int op, size_t n, const uint32_t* a, const uint
   // and c.stream (non-blocking) does not wait for the legacy default stream
   CK(cudaMemcpyAsync(da, a, bytes, cudaMemcpyHostToDevice, c.stream));
   CK(cudaMemcpyAsync(db, b, bytes, cudaMemcpyHostToDevice, c.stream));
-  unsigned nb = (unsigned)((n + 127) / 128);
-  if (curve == EB200_CURVE_SECP256K1) k256_selftest_fe_kernel<<<nb, 128, 0, c.stream>>>(op, n, da, db, dout);
-  else if (curve == EB200_CURVE_ED25519 || curve == EB200_CURVE_CURVE25519) f25_selftest_kernel<<<nb, 128, 0, c.stream>>>(op, n, da, db, dout);
-  else {
-#define EB_ST(C) (sw_selftest_fe_kernel<C><<<nb, 128, 0, c.stream>>>(op, n, da, db, dout), 0)
-    (void)SW_DISPATCH(curve, EB_ST);
-#undef EB_ST
-  }
+  const unsigned nb = blocks128(n);
+  if (curve == EB200_CURVE_ED25519 || curve == EB200_CURVE_CURVE25519) f25_selftest_kernel<<<nb, 128, 0, c.stream>>>(op, n, da, db, dout);
+  else with_curve(curve, [&](auto cv) {
+    typedef decltype(cv) T;
+    if constexpr (is_k256<T>) k256_selftest_fe_kernel<<<nb, 128, 0, c.stream>>>(op, n, da, db, dout);
+    else if constexpr (!is_ed25519<T>) sw_selftest_fe_kernel<typename T::C><<<nb, 128, 0, c.stream>>>(op, n, da, db, dout);
+    return EB200_OK;
+  });
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, c.stream));
   CK(cudaStreamSynchronize(c.stream));
@@ -2067,14 +1937,13 @@ int eb200_selftest_fe(int curve, int op, size_t n, const uint32_t* a, const uint
 
 int eb200_selftest_gtab_dims(int curve, int* windows, int* entries, int* wbits) {
   if (!windows || !entries || !wbits) return EB200_ERR_ARG;
-  if (curve == EB200_CURVE_SECP256K1) { *windows = GTAB_WINDOWS; *entries = GTAB_ENTRIES; *wbits = GTAB_W; }
-  else if (curve_len(curve)) {
-#define EB_DIM(C) (*windows = SW<C>::GWINDOWS, *entries = SW<C>::GENTRIES, *wbits = SW<C>::GW, 0)
-    (void)SW_DISPATCH(curve, EB_DIM);
-#undef EB_DIM
-  }
-  else return EB200_ERR_UNSUPPORTED;
-  return EB200_OK;
+  // ed25519 answers with the p224 geometry, as it always has (its own table is not in this layout)
+  return with_curve(curve == EB200_CURVE_ED25519 ? EB200_CURVE_P224 : curve, [&](auto cv) {
+    typedef decltype(cv) T;
+    if constexpr (is_k256<T>) { *windows = GTAB_WINDOWS; *entries = GTAB_ENTRIES; *wbits = GTAB_W; }
+    else if constexpr (!is_ed25519<T>) { typedef SW<typename T::C> W; *windows = W::GWINDOWS; *entries = W::GENTRIES; *wbits = W::GW; }
+    return EB200_OK;
+  });
 }
 
 int eb200_selftest_gtab(int curve, uint32_t* out, size_t n_words) {

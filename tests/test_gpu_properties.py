@@ -176,10 +176,92 @@ def test_openssl_signatures_verify_and_forgeries_do_not(native, name):
         assert (g.verify_batch_der_packed(e2, ders, pub, fmt) == 0).all()
 
 
+# return codes with cuda:0 initialised (argument_cases(with_device=True)); nullK: NULL in argument K
+WITH_DEVICE = {
+    "eb200_curve_add_batch": {"desc_null": -3, "n0": 0, "null2": -3, "null3": -3, "null4": -3, "null5": -3},
+    "eb200_curve_dbl_batch": {"desc_null": -3, "n0": 0, "null2": -3, "null3": -3, "null4": -3},
+    "eb200_curve_mul_add_batch": {"desc_null": -3, "n0": 0, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null7": -3, "null8": -3},
+    "eb200_curve_mul_batch": {"desc_null": -3, "n0": 0, "null2": -3, "null4": -3, "null5": -3, "null6": -3},
+    "eb200_curve_validate_batch": {"desc_null": -3, "n0": 0, "null2": -3, "null3": -3},
+    "eb200_ec_keygen_batch": {"curve77": -5, "n0": 0, "null2": -3, "null4": -3, "null6": -3, "null7": 0, "null8": -3},
+    "eb200_ecdh_derive_batch": {"curve77": -5, "n0": 0, "null2": -3, "null3": -3, "null4": -3, "null5": -3},
+    "eb200_ecdsa_recover_batch": {"curve77": -5, "n0": 0, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3, "null7": -3},
+    "eb200_ecdsa_sign_batch": {"curve77": -5, "n0": 0, "null2": -3, "null3": -3, "null5": -3, "null6": -3, "null7": -3, "null8": -3},
+    "eb200_ecdsa_sign_batch_k": {"curve77": -5, "n0": 0, "null2": -3, "null3": -3, "null4": -3, "null6": -3, "null7": -3, "null8": -3, "null9": -3},
+    "eb200_ecdsa_sign_batch_pers": {"curve77": -5, "n0": 0, "null10": -3, "null2": -3, "null3": -3, "null4": -3, "null7": -3, "null8": -3, "null9": -3},
+    "eb200_ecdsa_verify_batch": {"curve77": -5, "fmt9": -5, "n0": 0, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null7": -3},
+    "eb200_ecdsa_verify_batch_der": {"curve77": -5, "fmt9": -5, "n0": 0, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null7": -3},
+    "eb200_ecdsa_verify_batch_dev": {"curve77": -5, "fmt9": -5, "n0": 0, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null7": -3, "null8": -3, "null9": -4},
+    "eb200_eddsa_sign_batch": {"n0": 0, "null1": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3},
+    "eb200_eddsa_verify_batch": {"n0": 0, "null1": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3},
+    "eb200_eddsa_verify_batch_dev": {"n0": 0, "null1": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3, "null7": -4},
+    "eb200_eddsa_verify_batch_msgs": {"n0": 0, "null1": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3},
+    "eb200_last_timing": {"null0": -3},
+    "eb200_mul_add_batch": {"curve77": -5, "n0": 0, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3},
+    "eb200_scalar_mul_batch": {"curve77": -5, "n0": 0, "null2": -3, "null3": 0, "null4": -3, "null5": -3},
+    "eb200_selftest_fe": {"curve77": -5, "n0": 0},
+    "eb200_selftest_gtab": {"curve77": -5},
+    "eb200_selftest_gtab_dims": {"curve77": -5, "null1": -3, "null2": -3, "null3": -3},
+    "eb200_x25519_derive_batch": {"n0": 0, "null1": -3, "null2": -3, "null3": -3, "null4": -3},
+    "eb200_x25519_derive_batch_dev": {"n0": 0, "null1": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -4},
+    "eb200_x25519_mul_batch": {"n0": 0, "null1": -3, "null2": -3, "null3": -3, "null4": -3},
+}
+# eb200_timing.launches after each call of launch_cases(): kernels launched per entry point x curve x mode
+# (curve ids as in the header; fmtF: public-key format; 262921 items and `chunked`: cut into chunks)
+LAUNCHES = {
+    "curve_add/p256": 1, "curve_add/p384": 1, "curve_add/p521": 1,
+    "curve_dbl/p256": 1, "curve_dbl/p384": 1, "curve_dbl/p521": 1,
+    "curve_mul/p256": 1, "curve_mul/p384": 1, "curve_mul/p521": 1,
+    "curve_mul_add/p256": 1, "curve_mul_add/p384": 1, "curve_mul_add/p521": 1,
+    "curve_validate/p256": 1, "curve_validate/p384": 1, "curve_validate/p521": 1,
+    "derive/1": 3, "derive/2": 3, "derive/3": 3, "derive/4": 1, "derive/6": 3, "derive/7": 3, "derive/8": 3,
+    "eddsa_sign/pub0": 1, "eddsa_sign/pub1": 1,
+    "eddsa_verify/256": 1, "eddsa_verify/262921": 5,
+    "eddsa_verify_dev": 1,
+    "eddsa_verify_msgs/256": 2, "eddsa_verify_msgs/262921": 10,
+    "keygen/1/pers0": 2, "keygen/1/pers1": 2, "keygen/2/pers0": 2, "keygen/2/pers1": 2, "keygen/3/pers0": 2,
+    "keygen/3/pers1": 2, "keygen/4/pers0": 2, "keygen/4/pers1": 2, "keygen/6/pers0": 2, "keygen/6/pers1": 2,
+    "keygen/7/pers0": 2, "keygen/7/pers1": 2, "keygen/8/pers0": 2, "keygen/8/pers1": 2,
+    "mul/1/points0": 1, "mul/1/points1": 3, "mul/2/points0": 1, "mul/2/points1": 3, "mul/3/points0": 1,
+    "mul/3/points1": 3, "mul/4/points0": 1, "mul/4/points1": 1, "mul/6/points0": 1, "mul/6/points1": 3,
+    "mul/7/points0": 1, "mul/7/points1": 3, "mul/8/points0": 1, "mul/8/points1": 3,
+    "mul_add/1": 3, "mul_add/2": 3, "mul_add/3": 3, "mul_add/4": 1, "mul_add/6": 3, "mul_add/7": 3, "mul_add/8": 3,
+    "recover/1": 2, "recover/2": 2, "recover/3": 2, "recover/6": 2, "recover/7": 2, "recover/8": 2,
+    "sign/1/flags0": 3, "sign/1/flags1": 3, "sign/2/flags0": 3, "sign/2/flags1": 3, "sign/3/flags0": 3,
+    "sign/3/flags1": 3, "sign/4/flags0": 1, "sign/4/flags1": 1, "sign/6/flags0": 3, "sign/6/flags1": 3,
+    "sign/7/flags0": 3, "sign/7/flags1": 3, "sign/8/flags0": 3, "sign/8/flags1": 3,
+    "sign_k/1": 3, "sign_k/2": 3, "sign_k/3": 3, "sign_k/4": 1, "sign_k/6": 3, "sign_k/7": 3, "sign_k/8": 3,
+    "sign_pers/1/len0": 1, "sign_pers/1/len5": 1, "sign_pers/2/len0": 1, "sign_pers/2/len5": 1, "sign_pers/3/len0": 1,
+    "sign_pers/3/len5": 1, "sign_pers/4/len0": 1, "sign_pers/4/len5": 1, "sign_pers/6/len0": 1, "sign_pers/6/len5": 1,
+    "sign_pers/7/len0": 1, "sign_pers/7/len5": 1, "sign_pers/8/len0": 1, "sign_pers/8/len5": 1,
+    "verify/1/chunked": 15, "verify/1/fmt0": 3, "verify/1/fmt1": 4, "verify/1/fmt2": 4, "verify/2/chunked": 15,
+    "verify/2/fmt0": 3, "verify/2/fmt1": 4, "verify/2/fmt2": 4, "verify/3/fmt0": 3, "verify/3/fmt1": 4,
+    "verify/3/fmt2": 4, "verify/4/fmt0": 1, "verify/4/fmt1": 2, "verify/4/fmt2": 2, "verify/6/fmt0": 3,
+    "verify/6/fmt1": 4, "verify/6/fmt2": 4, "verify/7/fmt0": 3, "verify/7/fmt1": 4, "verify/7/fmt2": 4,
+    "verify/8/fmt0": 3, "verify/8/fmt1": 4, "verify/8/fmt2": 4,
+    "verify_der/1/fmt0": 4, "verify_der/1/fmt1": 5, "verify_der/1/fmt2": 5, "verify_der/2/fmt0": 4,
+    "verify_der/2/fmt1": 5, "verify_der/2/fmt2": 5, "verify_der/3/fmt0": 4, "verify_der/3/fmt1": 5,
+    "verify_der/3/fmt2": 5, "verify_der/4/fmt0": 2, "verify_der/4/fmt1": 3, "verify_der/4/fmt2": 3,
+    "verify_der/6/fmt0": 4, "verify_der/6/fmt1": 5, "verify_der/6/fmt2": 5, "verify_der/7/fmt0": 4,
+    "verify_der/7/fmt1": 5, "verify_der/7/fmt2": 5, "verify_der/8/fmt0": 4, "verify_der/8/fmt1": 5,
+    "verify_der/8/fmt2": 5,
+    "verify_dev/1/fmt0": 3, "verify_dev/1/fmt1": 4, "verify_dev/1/fmt2": 4, "verify_dev/2/fmt0": 3,
+    "verify_dev/2/fmt1": 4, "verify_dev/2/fmt2": 4, "verify_dev/3/fmt0": 3, "verify_dev/3/fmt1": 4,
+    "verify_dev/3/fmt2": 4, "verify_dev/4/fmt0": 1, "verify_dev/4/fmt1": 2, "verify_dev/4/fmt2": 2,
+    "verify_dev/6/fmt0": 3, "verify_dev/6/fmt1": 4, "verify_dev/6/fmt2": 4, "verify_dev/7/fmt0": 3,
+    "verify_dev/7/fmt1": 4, "verify_dev/7/fmt2": 4, "verify_dev/8/fmt0": 3, "verify_dev/8/fmt1": 4,
+    "verify_dev/8/fmt2": 4,
+    "x25519_derive/256": 1, "x25519_derive/262921": 5,
+    "x25519_derive_dev": 1,
+    "x25519_mul/256": 1, "x25519_mul/262921": 5,
+}
+
+
 def test_c_abi_argument_and_error_behaviour(native):
     """The boundary's own contract (include/elliptic_b200.h): empty batches succeed without touching the output,
     NULL pointers and unknown curves / formats come back as error codes, never as a crash, and the library
-    stays usable afterwards."""
+    stays usable afterwards.  Every entry point's codes for those cases and its launch count per curve and mode
+    are pinned in WITH_DEVICE and LAUNCHES."""
     from elliptic_b200 import _native as nat
     lib = nat.init(0)
     z = np.zeros((4, 64), np.uint8); st = np.full(4, 0xEE, np.uint8)
@@ -194,6 +276,21 @@ def test_c_abi_argument_and_error_behaviour(native):
     # all-zero inputs are legal inputs: r = s = 0 -> FALSE for every item
     assert lib.eb200_ecdsa_verify_batch(1, 4, z.ctypes.data, z.ctypes.data, z.ctypes.data, z.ctypes.data, 0, st.ctypes.data) == nat.OK
     assert (st == 0).all()
+    # every entry point: n == 0, NULL pointers, unknown curves / formats
+    from abi_cases import argument_cases, launch_cases
+    cases, _keep = argument_cases(with_device=True)
+    got = {}
+    for cid, call in cases:
+        name, tag = cid.split("/")
+        got.setdefault(name, {})[tag] = call(lib)
+    assert got == WITH_DEVICE
+    # the kernels each call launches, counted where they are launched
+    cases, _keep = launch_cases()
+    got = {}
+    for cid, call in cases:
+        assert call(lib) == nat.OK, cid
+        got[cid] = nat.last_timing()["launches"]
+    assert got == LAUNCHES, {k: (v, LAUNCHES.get(k)) for k, v in got.items() if LAUNCHES.get(k) != v}
 
 
 def test_chunked_host_pipeline_equals_single_launch(native):
