@@ -210,6 +210,22 @@ static napi_value EcdsaRecoverBatch(napi_env env, napi_callback_info info) {
   return res;
 }
 
+/* ecdsaRecoveryParamBatch(curveId, e, r, s, pubXY) -> {recid, status}   (getKeyRecoveryParam, ec/index.js:261-278) */
+static napi_value EcdsaRecoveryParamBatch(napi_env env, napi_callback_info info) {
+  ARGS(5); I32(0, curve); BUF(1, e, le); BUF(2, r, lr); BUF(3, s, ls); BUF(4, q, lq);
+  size_t len = field_len(curve);
+  if (!len) return fail(env, EB200_ERR_UNSUPPORTED);
+  size_t n = le / len;
+  if (le != n * len || lr != le || ls != le || lq != 2 * le) return fail(env, EB200_ERR_ARG);
+  uint8_t *id, *st;
+  napi_value ai = out_u8(env, n, &id), ast = out_u8(env, n, &st);
+  int rc = eb200_ecdsa_recovery_param_batch(curve, n, e, r, s, q, id, st);
+  if (rc) return fail(env, rc);
+  napi_value res = obj(env);
+  SET(res, "recid", ai); SET(res, "status", ast);
+  return res;
+}
+
 /* mulAddBatch(curveId, k1 | null, k2, points | null) -> {points, status}
  * k1 null: Point.mul (short.js:422-432, edwards.js:362-367); points null: G.mul; both: G.mulAdd(k1, P, k2) */
 static napi_value MulAddBatch(napi_env env, napi_callback_info info) {
@@ -313,7 +329,8 @@ static napi_value Register(napi_env env, napi_value exports) {
   static const struct { const char* name; napi_callback cb; } fns[] = {
       {"init", Init}, {"ecdsaVerifyBatch", EcdsaVerifyBatch}, {"ecdsaVerifyBatchAsync", EcdsaVerifyBatchAsync},
       {"ecdsaVerifyBatchDer", EcdsaVerifyBatchDer}, {"ecdsaSignBatch", EcdsaSignBatch}, {"ecKeygenBatch", EcKeygenBatch},
-      {"ecdsaRecoverBatch", EcdsaRecoverBatch}, {"mulAddBatch", MulAddBatch}, {"ecdhDeriveBatch", EcdhDeriveBatch},
+      {"ecdsaRecoverBatch", EcdsaRecoverBatch}, {"ecdsaRecoveryParamBatch", EcdsaRecoveryParamBatch},
+      {"mulAddBatch", MulAddBatch}, {"ecdhDeriveBatch", EcdhDeriveBatch},
       {"curveOpBatch", CurveOpBatch}, {"eddsaVerifyBatch", EddsaVerifyBatch}, {"eddsaSignBatch", EddsaSignBatch},
       {"x25519Batch", X25519Batch}};
   for (unsigned i = 0; i < sizeof fns / sizeof fns[0]; i++) {

@@ -2,7 +2,8 @@
 // Drop-in for require('elliptic'): every export of lib/elliptic.js:5-13 is the reference's own object
 // (single-item behaviour unchanged); the batch entry points below are added on the same prototypes and
 // run on the GPU through the N-API addon -> libelliptic_b200.so (include/elliptic_b200.h):
-//   EC#verifyBatch / verifyBatchAsync / signBatch / genKeyPairBatch / recoverPubKeyBatch / deriveBatch
+//   EC#verifyBatch / verifyBatchAsync / signBatch / genKeyPairBatch / recoverPubKeyBatch / getKeyRecoveryParamBatch /
+//   deriveBatch
 //   EDDSA#verifyBatch / signBatch
 //   curve.short#mulBatch / mulAddBatch / addBatch / dblBatch / validateBatch   (any parameters, presets take the tuned kernels)
 //   curve.edwards#mulBatch / mulAddBatch (ed25519), curve.mont#mulBatch (curve25519)
@@ -170,6 +171,38 @@ elliptic.ec.prototype.recoverPubKeyBatch = function recoverPubKeyBatch(msgs, sig
     if (res.status[i] === 7) out.push(this.curve.point(null, null));
     else if (res.status[i] !== 1) throw new Error(THROW[res.status[i]]);
     else out.push(this.curve.point(new BN(res.pub.subarray(2 * len * i, 2 * len * i + len)), new BN(res.pub.subarray(2 * len * i + len, 2 * len * (i + 1)))));
+  }
+  return out;
+};
+
+// EC#getKeyRecoveryParamBatch(msgs, sigs, Qs[, enc]) -> Array<number>   (getKeyRecoveryParam, ec/index.js:261-278); throws
+// 'Unable to find valid recovery factor' where a loop over getKeyRecoveryParam would.  The reference's own call answers
+// wherever recoverPubKeyBatch falls back, and for signatures that carry a recoveryParam or a Q at infinity.
+elliptic.ec.prototype.getKeyRecoveryParamBatch = function getKeyRecoveryParamBatch(msgs, sigs, Qs, enc) {
+  var id = curveId(this), self = this;
+  var len = this.curve.p.byteLength(), n = msgs.length;
+  var Signature = this.sign('00', '01').constructor;
+  var S = sigs.map(function(s) { return new Signature(s, enc); });
+  var one = function(i) { return self.getKeyRecoveryParam(msgs[i], sigs[i], Qs[i], enc); };
+  if (id === undefined || this.curve.type !== 'short' || S.some(function(s) { return s.r.byteLength() > len; }))
+    return msgs.map(function(_, i) { return one(i); });
+  var todo = [];
+  S.forEach(function(s, i) { if (s.recoveryParam === null && !Qs[i].isInfinity()) todo.push(i); });
+  var res = null;
+  if (todo.length) {
+    init();
+    var e = pack(todo, len, function(i) { return be(new BN(msgs[i]).umod(self.n), len); });
+    var r = pack(todo, len, function(i) { return be(S[i].r, len); });
+    var s = pack(todo, len, function(i) { return be(S[i].s.umod(self.n), len); });
+    var q = pack(todo, 2 * len, function(i) { return be(Qs[i].getX(), len).concat(be(Qs[i].getY(), len)); });
+    res = native.ecdsaRecoveryParamBatch(id, e, r, s, q);
+  }
+  var out = new Array(n), k = 0;
+  for (var i = 0; i < n; i++) {
+    if (k < todo.length && todo[k] === i) {
+      if (res.status[k] !== 1) throw new Error('Unable to find valid recovery factor');
+      out[i] = res.recid[k++];
+    } else out[i] = one(i);
   }
   return out;
 };

@@ -24,15 +24,10 @@
 #include "ed25519_body.cuh"
 #include "ed25519_ec.cuh"
 #include "sw_runtime.cuh"
+#include "kernel_bounds.h"
+#include "recovery_param.h"
 
 using namespace eb;
-
-#ifndef EB_VERIFY_BLOCK
-#define EB_VERIFY_BLOCK 128
-#endif
-#ifndef EB_VERIFY_MINBLOCKS
-#define EB_VERIFY_MINBLOCKS 3
-#endif
 
 // ---------------------------------------------------------------------------
 // secp256k1 kernels
@@ -236,12 +231,6 @@ __global__ void __launch_bounds__(128) sw_prep_kernel(size_t N, const uint8_t* _
   size_t T = (size_t)gridDim.x * blockDim.x;
   SW<C>::prep_thread(tid, T, N, e, r, s, ws, scratch);
 }
-#ifndef EB_SW_MINBLOCKS_BIG
-#define EB_SW_MINBLOCKS_BIG 2     // 12- and 18-limb curves (p384, p521): 255 registers
-#endif
-#ifndef EB_SW_MINBLOCKS8
-#define EB_SW_MINBLOCKS8 4        // 8-limb curves (p256, p224): four 128-thread blocks per SM (128 registers, a little
-#endif                            // spill) measured faster than three blocks / 168 registers at N = 2^20
 template <class C>
 __global__ void __launch_bounds__(128, (C::N <= 8) ? EB_SW_MINBLOCKS8 : EB_SW_MINBLOCKS_BIG)
 sw_verify_kernel(size_t N, const uint8_t* __restrict__ pub, const uint8_t* __restrict__ r, const u32* __restrict__ ws,
@@ -1961,6 +1950,46 @@ int eb200_selftest_gtab(int curve, uint32_t* out, size_t n_words) {
   CK(cudaMemcpyAsync(out, c.gtab[curve], words * 4, cudaMemcpyDeviceToHost, c.stream));
   CK(cudaStreamSynchronize(c.stream));
   return EB200_OK;
+}
+
+}  // extern "C"
+
+// ---- EC.getKeyRecoveryParam ----------------------------------------------------------------------------------------
+// The kernels are in recovery_param.cu (see there why); this side stages the buffers and runs them like recover_on.
+static int recovery_param_on(Ctx& c, int curve, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
+                             const uint8_t* q_xy, uint8_t* out_recid, uint8_t* status) {
+  int rc = ensure_table(c, curve);
+  if (rc) return rc;
+  const size_t len = curve_len(curve);
+  const WsLayout W = ws_layout(curve, n);
+  if ((rc = grow(&c.d_in, &c.d_in_cap, n * (5 * len + 1) + 256))) return rc;
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, W.total))) return rc;
+  if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
+  uint8_t *d_e = c.d_in, *d_r = d_e + len * n, *d_s = d_r + len * n, *d_q = d_s + len * n, *d_id = d_q + 2 * len * n;
+  u32 *ws = (u32*)(c.d_ws + W.ws), *qtab = (u32*)(c.d_ws + W.qtab);
+  return run_single(c, {{d_e, e, len * n}, {d_r, r, len * n}, {d_s, s, len * n}, {d_q, q_xy, 2 * len * n}},
+    [&](Launch& L) {
+      const RecoveryParamArgs a{d_e, d_r, d_s, d_q, d_id, c.d_status, c.gtab[curve], ws, (u32*)(c.d_ws + W.scratch), qtab};
+      cudaError_t err = recovery_param_launch(curve, n, a, L.st, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END], &L.count);
+      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "recovery_param_launch");
+    },
+    {{out_recid, d_id, n}, {status, c.d_status, n}}, {}, false);     // nothing secret: no wipe
+}
+
+extern "C" {
+
+int eb200_ecdsa_recovery_param_batch(int curve, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
+                                     const uint8_t* q_xy, uint8_t* out_recid, uint8_t* status) {
+  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
+  if (n == 0) return EB200_OK;
+  if (!e || !r || !s || !q_xy || !out_recid || !status) return EB200_ERR_ARG;
+  if (curve == EB200_CURVE_ED25519) return EB200_ERR_UNSUPPORTED;      // cofactor 8: the one-multiplication identity fails
+  const size_t len = curve_len(curve);
+  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
+    return recovery_param_on(c, curve, m, e + lo * len, r + lo * len, s + lo * len, q_xy + lo * 2 * len, out_recid + lo,
+                             status + lo);
+  });
 }
 
 }  // extern "C"

@@ -35,6 +35,7 @@ namespace eb {
 enum : uint8_t {
   ST_FALSE = 0, ST_TRUE = 1, ST_THROW_INVALID_POINT = 2, ST_THROW_NOT_VALIDATED = 3,
   ST_NEEDS_HOST = 4, ST_THROW_ASSERT = 5, ST_THROW_POINT_FORMAT = 6, ST_INFINITY = 7, ST_THROW_SECOND_KEY = 8, ST_THROW_SIG_FORMAT = 9,
+  ST_THROW_NO_RECOVERY = 11,
 };
 
 // workspace layout (SoA, word-major so lanes are coalesced): PREP_WORDS words per item
@@ -153,6 +154,8 @@ EB_HD void prep_store(size_t i, size_t N, u32* u1, const u32* u2, u32 flags, u32
 // mode 0 (verify, ec/index.js:199-207): invert s; u1 = e/s, u2 = r/s; r, s outside [1, n-1] -> FALSE.
 // mode 1 (recoverPubKey, ec/index.js:250-258): invert r; u1 = -e/r, u2 = s/r; no range checks
 //         (r = 0 mod n gives rInv = 0 exactly like BN.invm, i.e. the point at infinity).
+// mode 2 (getKeyRecoveryParam, recovery_param_item): invert s mod n; u1 = e/s, u2 = (r mod n)/s; no range checks;
+//         s = 0 (mod n) -> FL_INVALID (recovery_param_cold_item decides those items).
 EB_HD void prep_thread(size_t tid, size_t T, size_t N, const uint8_t* e, const uint8_t* r,
                        const uint8_t* s, u32* ws, u32* scratch, int mode = 0) {
   u32 R2[8], one[8], nn[8];
@@ -175,6 +178,7 @@ EB_HD void prep_thread(size_t tid, size_t T, size_t N, const uint8_t* e, const u
       ok = !is_zero_n<8>(sm);
     } else {
       sc_mont_mul(sm, sv, R2);
+      if (mode == 2) ok = !is_zero_n<8>(sm);        // s mod n
     }
     if (!ok) invalid_mask |= 1u << j;
     cmov_n<8>(sm, one, !ok);
@@ -472,6 +476,43 @@ EB_HD uint8_t recover_item(size_t i, size_t N, const uint8_t* r, const uint8_t* 
   fe qx = fe_normalize(q.x), qy = fe_normalize(q.y);
   store_be<8>(out + 64 * i, qx.v);
   store_be<8>(out + 64 * i + 32, qy.v);
+  return ST_TRUE;
+}
+
+// EC.prototype.getKeyRecoveryParam (ec/index.js:261-278) with one double-scalar multiplication instead of its loop over
+// recoverPubKey.  The group has prime order, so for r, s != 0 (mod n): r^-1 (s R - e G) = Q  <=>  R = s^-1 (e G + r Q) = P.
+// prep_thread mode 2 leaves u1 = e/s, u2 = r/s, and the answer is read off P: x(P) = r mod p gives j = parity(y(P)),
+// x(P) = r + n (r < p - n) gives j = 2 + parity(y(P)), anything else (or P = O) no j.  P itself proves that pointFromX
+// finds that candidate.  recid: 1 byte per item, 0 unless ST_TRUE.  Status ST_TRUE, ST_THROW_NO_RECOVERY, or
+// ST_NEEDS_HOST for s = 0 (mod n), which recovery_param_cold_item (ecdsa_k256_sign.cuh) decides.
+EB_HD uint8_t recovery_param_item(size_t i, size_t N, const uint8_t* q, const uint8_t* r, const u32* ws, const u32* gtab,
+                                  u32* qtab, uint8_t* recid) {
+  recid[i] = 0;
+  ge_aff Q;
+  Q.x = fe_from_be(q + 64 * i);
+  Q.y = fe_from_be(q + 64 * i + 32);
+  if (!aff_on_curve(Q)) return ST_THROW_NO_RECOVERY;       // a recovered point is always on the curve
+  u32 rv[8], nn[8];
+  load_be<8>(rv, r + 32 * i);
+  K256N::n(nn);
+  if (is_zero_n<8>(rv) || eq_n<8>(rv, nn)) return ST_THROW_NO_RECOVERY;   // r = 0 (mod n): rInv = 0, every Q' is O
+  u32 flags = ws[(size_t)18 * N + i];
+  if (flags & FL_INVALID) return ST_NEEDS_HOST;             // s = 0 (mod n)
+  ge_jac acc = k256_dsm(i, N, Q, flags, ws, gtab, qtab);
+  if (fe_is_zero(acc.z)) return ST_THROW_NO_RECOVERY;
+  fe z2 = fe_sqr(acc.z);
+  u32 j = 0;
+  if (!fe_eq(acc.x, fe_mul(fe_from_be(r + 32 * i), z2))) {
+    const u32 pmn[8] = {0x2fc9baeeu, 0x402da172u, 0x50b75fc4u, 0x45512319u, 0x00000001u, 0, 0, 0};  // p mod n = p - n
+    if (geq_n<8>(rv, pmn)) return ST_THROW_NO_RECOVERY;    // no second candidate (ec/index.js:243)
+    fe rn;
+    add_n<8>(rn.v, rv, nn);
+    if (!fe_eq(acc.x, fe_mul(rn, z2))) return ST_THROW_NO_RECOVERY;
+    j = 2;
+  }
+  fe zi = fe_inv(acc.z);
+  if (fe_is_odd(fe_mul(fe_mul(acc.y, fe_sqr(zi)), zi))) j |= 1;
+  recid[i] = (uint8_t)j;
   return ST_TRUE;
 }
 

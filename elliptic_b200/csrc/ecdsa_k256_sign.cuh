@@ -111,6 +111,37 @@ EB_HD uint8_t k256_mul_g_item(size_t i, const uint8_t* k, const u32* gtab, uint8
   return ST_TRUE;
 }
 
+// getKeyRecoveryParam for the items recovery_param_item leaves as ST_NEEDS_HOST: s = 0, r != 0 (mod n).  There
+// s2 = s rInv = 0, so recoverPubKey(e, sig, j) returns s1 G = ((n - e) / r) G for every j whose candidate exists, and the
+// answer is the first such j when Q is that point.  Candidates exist as recover_item finds them: j = 0 (and 1) when
+// r is an x coordinate, j = 2 (and 3) when r + n < p is one.
+EB_HD uint8_t recovery_param_cold_item(size_t i, const uint8_t* e, const uint8_t* r, const uint8_t* q, const u32* gtab,
+                                       uint8_t* recid) {
+  u32 R2[8], nn[8], rv[8], ev[8], rm[8], rinv[8], k[8];
+  K256N::r2(R2); K256N::n(nn);
+  load_be<8>(rv, r + 32 * i);
+  load_be<8>(ev, e + 32 * i);
+  sc_mont_mul(rm, rv, R2);                        // r mod n, Montgomery form
+  sc_mont_inv(rinv, rm);
+  sc_mont_mul(k, ev, rinv);                       // e / r
+  if (is_zero_n<8>(k)) return ST_THROW_NO_RECOVERY;   // s1 = 0: every Q' is the point at infinity
+  sub_n<8>(k, nn, k);                             // (n - e) / r
+  ge_aff T = k256_mul_g(k, gtab);
+  if (!fe_eq(fe_from_be(q + 64 * i), T.x) || !fe_eq(fe_from_be(q + 64 * i + 32), T.y)) return ST_THROW_NO_RECOVERY;
+  const u32 pmn[8] = {0x2fc9baeeu, 0x402da172u, 0x50b75fc4u, 0x45512319u, 0x00000001u, 0, 0, 0};  // p mod n = p - n
+  for (u32 j = 0; j < 4; j += 2) {
+    if (j == 2 && geq_n<8>(rv, pmn)) break;       // 'Unable to find sencond key candinate'
+    fe x;
+    copy_n<8>(x.v, rv);
+    if (j == 2) add_n<8>(x.v, rv, nn);
+    fe seven = fe_zero(); seven.v[0] = 7;
+    fe y2 = fe_add(fe_mul(fe_sqr(x), x), seven);
+    fe y = fe_sqrt_candidate(y2);
+    if (fe_eq(fe_sqr(y), y2)) { recid[i] = (uint8_t)j; return ST_TRUE; }
+  }
+  return ST_THROW_NO_RECOVERY;
+}
+
 // One attempt of the loop body of ec/index.js:153-185 for a given nonce k (little-endian limbs, already
 // _truncateToN(k, true)'d): false = the reference `continue`s (k out of range, r = 0 or s = 0).
 EB_HD bool k256_sign_try(size_t i, const u32* k, const u32* ev, const u32* dv, u32 canonical, const u32* gtab,

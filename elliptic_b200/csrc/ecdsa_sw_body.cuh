@@ -436,6 +436,100 @@ struct SW {
     return 1;
   }
 
+  // getKeyRecoveryParam scalars (recovery_param_item): u1 = e / s, u2 = (r mod n) / s for r, s any values below
+  // 2^(8 LEN); s = 0 (mod n) is flagged FL_INVALID for the cold path.  One inversion per item, as prep_recover_item.
+  static EB_HD void prep_recovery_param_item(size_t i, size_t cnt_items, const uint8_t* e, const uint8_t* r,
+                                             const uint8_t* s, u32* ws) {
+    typedef typename S::fe sc;
+    const size_t LEN = C::LEN;
+    sc rv, sv, ev;
+    ldb(rv.v, r + LEN * i); ldb(sv.v, s + LEN * i); ldb(ev.v, e + LEN * i);
+    sc sm = S::to_mont(sv);                              // s mod n, Montgomery form
+    sc sinv = S::zero();
+    u32 flags = FL_INVALID;
+    if (!S::is_zero(sm)) { sinv = S::inv(sm); flags = 0; }
+    sc u1 = S::mul(ev, sinv);                            // e / s (plain; e < n)
+    sc u2 = S::mul(rv, sinv);                            // r / s (plain; r < R)
+    prep_store(i, cnt_items, u1.v, u2.v, flags, ws);
+  }
+
+  // EC.prototype.getKeyRecoveryParam (ec/index.js:261-278) with one double-scalar multiplication: the group has prime
+  // order, so for r, s != 0 (mod n), recoverPubKey(e, sig, j) = Q exactly when its candidate R_j equals
+  // P = s^-1 (e G + r Q) = u1 G + u2 Q.  x(P) = r mod p gives j = parity(y(P)); x(P) = r + n (r < p mod n) gives
+  // j = 2 + parity(y(P)); anything else (or P = O) no j.  P proves that pointFromX finds that candidate, Tonelli-Shanks
+  // included (it succeeds on every square).  recid 0 unless 1; 1 = found, 11 = 'Unable to find valid recovery factor',
+  // 4 = s = 0 (mod n), decided by recovery_param_cold_item.
+  static EB_HD uint8_t recovery_param_item(size_t i, size_t cnt_items, const uint8_t* q, const uint8_t* r, const u32* ws,
+                                           const u32* gtab, u32* qtab, uint8_t* recid) {
+    const size_t LEN = C::LEN;
+    recid[i] = 0;
+    aff Q = load_point(q, i);
+    if (!on_curve(Q)) return 11;                         // a recovered point is always on the curve
+    u32 rn[N];
+    ldb(rn, r + LEN * i);
+    reduce_scalar(rn);
+    if (is_zero_n<N>(rn)) return 11;                     // r = 0 (mod n): rInv = 0, every Q' is the point at infinity
+    u32 flags = ws[(size_t)(2 * N) * cnt_items + i];
+    if (flags & FL_INVALID) return 4;
+    jac acc = dsm(i, cnt_items, Q, flags, ws, gtab, qtab);
+    if (F::is_zero(acc.z)) return 11;
+    fe z2 = F::sqr(acc.z);
+    fe rp;
+    ldb(rp.v, r + LEN * i);
+    u32 j = 0;
+    if (!F::eq(acc.x, F::mul(F::to_mont(rp), z2))) {
+      u32 pmn[N]; C::p_minus_n(pmn);
+      if (geq_n<N>(rp.v, pmn)) return 11;                // no second candidate (ec/index.js:243)
+      u32 nmod[N]; n_limbs(nmod);
+      add_n<N>(rp.v, rp.v, nmod);                        // r + n < p
+      if (!F::eq(acc.x, F::mul(F::to_mont(rp), z2))) return 11;
+      j = 2;
+    }
+    fe y = F::from_mont(to_aff(acc).y);
+    recid[i] = (uint8_t)(j | (y.v[0] & 1));
+    return 1;
+  }
+
+  // pointFromX(x) does not throw (recover_item's test); x plain, reduced mod p here as toRed does
+  static EB_HD bool has_point_at(const fe& xr) {
+    fe x = F::to_mont(xr);
+    fe y2 = F::add(F::sub(F::mul(F::sqr(x), x), F::add(F::dbl(x), x)), C::b());
+    fe y;
+    if (sqrt_ref(y2, &y)) return false;
+    return F::eq(F::sqr(y), y2);
+  }
+
+  // The items recovery_param_item leaves as 4: s = 0, r != 0 (mod n).  recoverPubKey then returns s1 G = ((n - e) / r) G
+  // for every j whose candidate exists, so the answer is the first such j when Q is that point: j = 0 when r is an x
+  // coordinate, else j = 2 when r + n < p is one.
+  static EB_HD uint8_t recovery_param_cold_item(size_t i, const uint8_t* e, const uint8_t* r, const uint8_t* q,
+                                                const u32* gtab, uint8_t* recid) {
+    typedef typename S::fe sc;
+    const size_t LEN = C::LEN;
+    u32 nmod[N];
+    n_limbs(nmod);
+    sc rv, ev;
+    ldb(rv.v, r + LEN * i); ldb(ev.v, e + LEN * i);
+    sc k = S::mul(ev, S::inv(S::to_mont(rv)));          // e / r
+    if (S::is_zero(k)) return 11;                        // s1 = 0: every Q' is the point at infinity
+    sub_n<N>(k.v, nmod, k.v);                            // (n - e) / r
+    uint8_t kb[C::LEN], t[2 * C::LEN], qb[2 * C::LEN];
+    stb(kb, k.v);
+    mul_g_item(0, kb, gtab, t);
+    store_point(qb, 0, load_point(q, i));                // Q reduced mod p, as curve.point holds it
+    for (size_t b = 0; b < 2 * LEN; b++)
+      if (t[b] != qb[b]) return 11;
+    fe x;
+    ldb(x.v, r + LEN * i);
+    if (has_point_at(x)) { recid[i] = 0; return 1; }
+    u32 pmn[N];
+    C::p_minus_n(pmn);
+    if (geq_n<N>(x.v, pmn)) return 11;                   // 'Unable to find sencond key candinate'
+    add_n<N>(x.v, x.v, nmod);
+    if (has_point_at(x)) { recid[i] = 2; return 1; }
+    return 11;
+  }
+
   // G.mul(k) (short.js:422-427 -> _fixedNafMul, base.js:52-84): fixed table only
   static EB_HD uint8_t mul_g_item(size_t i, const uint8_t* k, const u32* gtab, uint8_t* out) {
     const size_t LEN = C::LEN;

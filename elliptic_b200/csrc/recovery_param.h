@@ -1,0 +1,19 @@
+// recovery_param.h -- the EC.getKeyRecoveryParam kernels (recovery_param.cu), launched by eb200.cu
+#pragma once
+#include <cuda_runtime.h>
+#include <stddef.h>
+#include <stdint.h>
+
+// Device buffers of one eb200_ecdsa_recovery_param_batch block: e, r, s (n x len) and q (n x 2 len) in; recid and
+// status (n bytes) out; the curve's fixed-base table; ws / scratch / qtab as ws_layout places them.
+struct RecoveryParamArgs {
+  const uint8_t *e, *r, *s, *q;
+  uint8_t *recid, *status;
+  const uint32_t* gtab;
+  uint32_t *ws, *scratch, *qtab;
+};
+
+// Launches prep, main and cold on `st` for a short preset, recording main_begin / main_end around the main kernel, and
+// adds the kernels launched to *launches.  Other curve ids launch nothing and return cudaErrorInvalidValue.
+cudaError_t recovery_param_launch(int curve, size_t n, const RecoveryParamArgs& a, cudaStream_t st, cudaEvent_t main_begin,
+                                  cudaEvent_t main_end, unsigned* launches);

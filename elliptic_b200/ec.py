@@ -60,6 +60,7 @@ _THROW_MSG = {
     nat.ST_THROW_POINT_FORMAT: "Unknown point format",
     nat.ST_THROW_SECOND_KEY: "Unable to find sencond key candinate",
     nat.ST_THROW_SIG_FORMAT: "Signature without r or s",
+    nat.ST_THROW_NO_RECOVERY: "Unable to find valid recovery factor",
 }
 
 
@@ -441,6 +442,60 @@ class EC:
         pts, st = self.recover_pub_key_batch([msg], [signature], [j], enc)
         if st[0] in (nat.ST_TRUE, nat.ST_INFINITY):
             return pts[0]
+        raise EllipticError(_THROW_MSG.get(int(st[0]), "status %d" % int(st[0])))
+
+    def get_key_recovery_param_batch(self, msgs, sigs, qs, enc=None):
+        """Batch of EC.prototype.getKeyRecoveryParam (ec/index.js:261-278): per item the first j in 0..3 whose
+        recoverPubKey(msg, sig, j) equals Q.  msgs and sigs as recover_pub_key_batch takes them, qs the public points
+        as (x, y) pairs or {x, y} dicts (reduced mod p like curve.point).  A signature that carries a recoveryParam is
+        answered with it without any computation, as the reference does (ec/index.js:263-264).
+        Returns (js, statuses): js[i] is the parameter, or None where the reference throws
+        'Unable to find valid recovery factor' (status ST_THROW_NO_RECOVERY)."""
+        if self.name not in _SHORT:
+            raise EllipticError("get_key_recovery_param_batch: short curves only")
+        n, ln = len(msgs), self._len
+        js = [None] * n
+        st = np.zeros(n, np.uint8)
+        todo = []
+        rs = []
+        for i in range(n):
+            rv, sv = self._signature_enc(sigs[i], enc)                  # new Signature(signature, enc) may throw first
+            rp = sigs[i].get("recoveryParam") if isinstance(sigs[i], dict) else \
+                getattr(sigs[i], "recoveryParam", getattr(sigs[i], "recovery_param", None))
+            if rp is not None:
+                js[i], st[i] = rp, nat.ST_TRUE
+                continue
+            if qs[i] is None:
+                raise NeedsReferencePath("Q is the point at infinity")
+            if rv >> (8 * ln):
+                raise NeedsReferencePath("r does not fit the curve's field width")
+            todo.append(i)
+            rs.append((rv, sv))
+        if not todo:
+            return js, st
+        lib = nat.init(self._device)
+        m = len(todo)
+        e = np.zeros((m, ln), np.uint8); r = np.zeros((m, ln), np.uint8); s = np.zeros((m, ln), np.uint8)
+        for k, i in enumerate(todo):
+            rv, sv = rs[k]
+            ev = _bn(msgs[i]) if not isinstance(msgs[i], (bytes, bytearray, list, tuple)) else int.from_bytes(_to_array(msgs[i]), "big")
+            e[k] = np.frombuffer((ev % self.n).to_bytes(ln, "big"), np.uint8)
+            r[k] = np.frombuffer(rv.to_bytes(ln, "big"), np.uint8)
+            s[k] = np.frombuffer((sv % self.n).to_bytes(ln, "big"), np.uint8)
+        q = self._points([qs[i] for i in todo])
+        rid = np.zeros(m, np.uint8); sub = np.zeros(m, np.uint8)
+        nat.check(lib.eb200_ecdsa_recovery_param_batch(self._c["id"], m, e.ctypes.data, r.ctypes.data, s.ctypes.data,
+                                                       q.ctypes.data, rid.ctypes.data, sub.ctypes.data))
+        for k, i in enumerate(todo):
+            st[i] = sub[k]
+            js[i] = int(rid[k]) if sub[k] == nat.ST_TRUE else None
+        return js, st
+
+    def get_key_recovery_param(self, e, signature, Q, enc=None):
+        """EC.prototype.getKeyRecoveryParam (ec/index.js:261-278): the parameter, or raises like the reference."""
+        js, st = self.get_key_recovery_param_batch([e], [signature], [Q], enc)
+        if st[0] == nat.ST_TRUE:
+            return js[0]
         raise EllipticError(_THROW_MSG.get(int(st[0]), "status %d" % int(st[0])))
 
     # ---- curve.point(...).mul / mulAdd batches (short.js:422-441) ---------------------------------------------

@@ -46,6 +46,7 @@ extern "C" {
 #define EB200_ST_THROW_SIG_FORMAT 9     /* threw Error('Signature without r or s')  ec/signature.js:15 (DER rejected by _importDER) */
 #define EB200_ST_RETRY 10               /* (sign with caller nonces) the reference's loop `continue`s: k outside [2, n-2], r = 0 or s = 0;
                                            the caller supplies its next k(iter), ec/index.js:153-185 */
+#define EB200_ST_THROW_NO_RECOVERY 11   /* (getKeyRecoveryParam) threw Error('Unable to find valid recovery factor')  ec/index.js:277 */
 
 /* curve ids (names of lib/elliptic/curves.js presets) */
 #define EB200_CURVE_SECP256K1 1
@@ -137,6 +138,18 @@ int eb200_ecdsa_sign_batch(int curve, size_t n, const uint8_t* e, const uint8_t*
  * status: TRUE (point written), INFINITY, THROW_INVALID_POINT (pointFromX, short.js:195), THROW_SECOND_KEY. */
 int eb200_ecdsa_recover_batch(int curve, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
                               const uint8_t* recid, uint8_t* out_xy, uint8_t* status);
+
+/* Batch of EC.prototype.getKeyRecoveryParam (lib/elliptic/ec/index.js:261-278) on the six short presets: the first j in
+ * 0..3 whose recoverPubKey(e, sig, j) equals Q.  One double-scalar multiplication per item instead of up to four
+ * recoveries: the groups have prime order, so r^-1 (s R - e G) = Q exactly when R = s^-1 (e G + r Q).
+ *   e, r, s : n x len as eb200_ecdsa_recover_batch takes them (e reduced mod n; r, s any value below 2^(8 len))
+ *   q_xy    : n x 2len public points x || y big-endian, reduced mod p like curve.point; not validated (an off-curve Q
+ *             never equals a recovered point)
+ *   out_recid : n bytes, the parameter 0..3 (0 unless status is TRUE)
+ * status: TRUE or THROW_NO_RECOVERY.  The caller answers a signature that already carries its recoveryParam
+ * (ec/index.js:263-264).  ed25519: EB200_ERR_UNSUPPORTED, as recover. */
+int eb200_ecdsa_recovery_param_batch(int curve, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
+                                     const uint8_t* q_xy, uint8_t* out_recid, uint8_t* status);
 
 /* Batch of BasePoint.mul (lib/elliptic/curve/short.js:422-432) on secp256k1 / p256 / p384 (len = 32/32/48):
  *   k         : n x len big-endian scalars, any value below 2^(8 len) (the reference does not reduce them)
