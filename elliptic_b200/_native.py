@@ -6,6 +6,8 @@ CUDA device is usable, every compute call raises.
 import ctypes
 import os
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # EB200_LIB lets the tuning scripts load an alternative build of the same library
 LIB_PATH = os.environ.get("EB200_LIB") or os.path.join(_HERE, "libelliptic_b200.so")
@@ -38,6 +40,11 @@ class Timing(ctypes.Structure):
 
 class ShortCurveDesc(ctypes.Structure):
     _fields_ = [("len", ctypes.c_uint32), ("p", ctypes.c_void_p), ("a", ctypes.c_void_p), ("b", ctypes.c_void_p)]
+
+
+def short_curve(pab):
+    """The eb200_short_curve over the rows p, a, b of a (3, len) uint8 array, which the caller keeps alive."""
+    return ShortCurveDesc(pab.shape[1], *(row.ctypes.data for row in pab))
 
 
 class NativeError(RuntimeError):
@@ -103,6 +110,12 @@ def check(rc):
     if rc != OK:
         lib = load()
         raise NativeError("%s [%s]" % (lib.eb200_strerror(rc).decode(), lib.eb200_last_error().decode()))
+
+
+def call(fn, *args):
+    """fn(*args) with every numpy array passed as the address of its data (the caller keeps it contiguous) and None
+    as NULL; raises NativeError unless fn returns OK."""
+    check(fn(*(a.ctypes.data if isinstance(a, np.ndarray) else a for a in args)))
 
 
 _inited = set()

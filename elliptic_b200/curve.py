@@ -6,12 +6,10 @@ test (test/curve-test.js:9-22).  Points are (x, y) pairs (ints / hex / byte arra
 them); `None` stands for the point at infinity in results.  Every method takes and returns whole batches and runs
 on the GPU (include/elliptic_b200.h: eb200_curve_*_batch); the named presets have their own tuned entry points in
 elliptic_b200.ec.EC (mul_batch, mul_add_batch, g_mul_batch)."""
-import ctypes
-
 import numpy as np
 
 from . import _native as nat
-from .ec import EllipticError, NeedsReferencePath, _bn
+from .ec import EllipticError, NeedsReferencePath, _bn, _pack, _pack_points, _unpack
 
 
 class ShortCurve:
@@ -23,20 +21,16 @@ class ShortCurve:
             raise EllipticError("ShortCurve: p wider than 576 bits is not supported")
         self.len = max(1, (self.p.bit_length() + 7) // 8)
         self._device = device
-        self._bufs = [np.frombuffer((v % self.p).to_bytes(self.len, "big"), np.uint8).copy() for v in (self.p, self.a, self.b)]
-        self._bufs[0] = np.frombuffer(self.p.to_bytes(self.len, "big"), np.uint8).copy()
-        self._desc = nat.ShortCurveDesc(self.len, self._bufs[0].ctypes.data, self._bufs[1].ctypes.data, self._bufs[2].ctypes.data)
+        self._pab = _pack([self.p, self.a % self.p, self.b % self.p], self.len)
+        self._desc = nat.short_curve(self._pab)
 
     # ---- packing --------------------------------------------------------------------------------------------
     def _pts(self, pts):
-        out = np.zeros((len(pts), 2 * self.len), np.uint8)
-        for i, pt in enumerate(pts):
+        def finite(pt):
             if pt is None:
                 raise EllipticError("the point at infinity is not accepted as a batch input")
-            x, y = (pt["x"], pt["y"]) if isinstance(pt, dict) else pt
-            out[i, :self.len] = np.frombuffer((_bn(x) % self.p).to_bytes(self.len, "big"), np.uint8)
-            out[i, self.len:] = np.frombuffer((_bn(y) % self.p).to_bytes(self.len, "big"), np.uint8)
-        return out
+            return pt
+        return _pack_points(map(finite, pts), self.p, self.len)
 
     def _scalars(self, ks):
         vals = [_bn(k) for k in ks]
@@ -45,14 +39,13 @@ class ShortCurve:
         klen = max(1, max((v.bit_length() + 7) // 8 for v in vals)) if vals else 1
         if klen > 128:
             raise NeedsReferencePath("scalar wider than 1024 bits")
-        return np.frombuffer(b"".join(v.to_bytes(klen, "big") for v in vals), np.uint8).reshape(len(vals), klen).copy(), klen
+        return _pack(vals, klen), klen
 
-    def _result(self, out, st):
-        if bool((st == nat.ST_NEEDS_HOST).any()):
-            raise NeedsReferencePath("point %d is not on the curve; the reference does not validate it" % int(np.flatnonzero(st == nat.ST_NEEDS_HOST)[0]))
-        ln = self.len
-        return [(int.from_bytes(out[i, :ln].tobytes(), "big"), int.from_bytes(out[i, ln:].tobytes(), "big")) if st[i] == nat.ST_TRUE else None
-                for i in range(len(st))]
+    def _run(self, fn, n, *args):
+        """fn(desc, n, *args, out_xy, status) -> the n result points (None = infinity)."""
+        out = np.zeros((n, 2 * self.len), np.uint8); st = np.zeros(n, np.uint8)
+        nat.call(fn, self._desc, n, *args, out, st)
+        return _unpack(out, self.len, st, needs_host=True)
 
     # ---- batch entry points ---------------------------------------------------------------------------------
     def mul_batch(self, points, ks):
@@ -60,10 +53,7 @@ class ShortCurve:
         lib = nat.init(self._device)
         pts = self._pts(points)
         k, klen = self._scalars(ks)
-        n = len(pts)
-        out = np.zeros((n, 2 * self.len), np.uint8); st = np.zeros(n, np.uint8)
-        nat.check(lib.eb200_curve_mul_batch(ctypes.byref(self._desc), n, k.ctypes.data, klen, pts.ctypes.data, out.ctypes.data, st.ctypes.data))
-        return self._result(out, st)
+        return self._run(lib.eb200_curve_mul_batch, len(pts), k, klen, pts)
 
     def mul_add_batch(self, p1s, k1s, p2s, k2s):
         """[p1.mulAdd(k1, p2, k2)] = k1*p1 + k2*p2 (short.js:434-441)."""
@@ -71,35 +61,24 @@ class ShortCurve:
         a, b = self._pts(p1s), self._pts(p2s)
         kk, klen = self._scalars(list(k1s) + list(k2s))
         n = len(a)
-        k1, k2 = np.ascontiguousarray(kk[:n]), np.ascontiguousarray(kk[n:])
-        out = np.zeros((n, 2 * self.len), np.uint8); st = np.zeros(n, np.uint8)
-        nat.check(lib.eb200_curve_mul_add_batch(ctypes.byref(self._desc), n, k1.ctypes.data, a.ctypes.data, k2.ctypes.data, b.ctypes.data,
-                                                klen, out.ctypes.data, st.ctypes.data))
-        return self._result(out, st)
+        return self._run(lib.eb200_curve_mul_add_batch, n, kk[:n], a, kk[n:], b, klen)
 
     def add_batch(self, p1s, p2s):
         """[p1.add(p2)] (short.js:365-392)."""
         lib = nat.init(self._device)
         a, b = self._pts(p1s), self._pts(p2s)
-        n = len(a)
-        out = np.zeros((n, 2 * self.len), np.uint8); st = np.zeros(n, np.uint8)
-        nat.check(lib.eb200_curve_add_batch(ctypes.byref(self._desc), n, a.ctypes.data, b.ctypes.data, out.ctypes.data, st.ctypes.data))
-        return self._result(out, st)
+        return self._run(lib.eb200_curve_add_batch, len(a), a, b)
 
     def dbl_batch(self, points):
         """[p.dbl()] (short.js:394-412)."""
         lib = nat.init(self._device)
         a = self._pts(points)
-        n = len(a)
-        out = np.zeros((n, 2 * self.len), np.uint8); st = np.zeros(n, np.uint8)
-        nat.check(lib.eb200_curve_dbl_batch(ctypes.byref(self._desc), n, a.ctypes.data, out.ctypes.data, st.ctypes.data))
-        return self._result(out, st)
+        return self._run(lib.eb200_curve_dbl_batch, len(a), a)
 
     def validate_batch(self, points):
         """[curve.validate(p)] (short.js:206-216): booleans."""
         lib = nat.init(self._device)
         a = self._pts(points)
-        n = len(a)
-        st = np.zeros(n, np.uint8)
-        nat.check(lib.eb200_curve_validate_batch(ctypes.byref(self._desc), n, a.ctypes.data, st.ctypes.data))
+        st = np.zeros(len(a), np.uint8)
+        nat.call(lib.eb200_curve_validate_batch, self._desc, len(a), a, st)
         return [bool(v) for v in st]

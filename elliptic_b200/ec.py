@@ -7,7 +7,6 @@ point (SURVEY 8b: `EC#verifyBatch(msgs, sigs, pubs) -> Uint8Array`).  Parsing
 (hex / byte arrays / DER / SEC1) is done here exactly as the reference's JS
 does it; all curve arithmetic happens in libelliptic_b200.so on the GPU.
 """
-import ctypes
 import re
 
 import numpy as np
@@ -123,6 +122,76 @@ def _bn(v):
     return int.from_bytes(bytes(v), "big")
 
 
+def _msg_int(msg):
+    """`new BN(msg)` as recoverPubKey / getKeyRecoveryParam take the message: byte arrays big-endian, else as _bn."""
+    if isinstance(msg, (bytes, bytearray, list, tuple)):
+        return int.from_bytes(_to_array(msg), "big")
+    return _bn(msg)
+
+
+def _signature(sig, enc):
+    """new Signature(sig, enc) (ec/signature.js:8-22) -> (r, s)."""
+    if isinstance(sig, dict):
+        if not (sig.get("r") and sig.get("s")):
+            raise EllipticError("Signature without r or s")
+        return _bn(sig["r"]), _bn(sig["s"])
+    if hasattr(sig, "r") and hasattr(sig, "s"):
+        return int(sig.r), int(sig.s)
+    rs = parse_der(_to_array(sig, enc))
+    if rs is None:
+        raise EllipticError("Signature without r or s")
+    return rs
+
+
+def _pers(pers, pers_enc):
+    """The `pers` option after `persEnc` decoding (utf8 by default, ec/index.js:150) as a NUL-terminated uint8 array,
+    and its length; (None, 0) without one."""
+    if pers is None:
+        return None, 0
+    b = bytes(_to_array(pers, pers_enc or "utf8"))
+    return np.frombuffer(b + b"\x00", np.uint8), len(b)
+
+
+def _pack(vals, width, order="big"):
+    """Ints as an (n, width) uint8 array, one `width`-byte row each: the C ABI's item-major layout.  Each value is
+    encoded as `vals` yields it, so a generator that parses items stops at the first one that does not fit."""
+    return np.frombuffer(b"".join(v.to_bytes(width, order) for v in vals), np.uint8).reshape(-1, width)
+
+
+def _pack_points(pts, p, ln):
+    """curve.point(x, y) for (x, y) pairs or {x, y} dicts (short.js:251-271): an (n, 2 ln) array of x || y,
+    coordinates reduced mod p, not validated."""
+    xy = ((pt["x"], pt["y"]) if isinstance(pt, dict) else pt for pt in pts)
+    return _pack((_bn(c) % p for x, y in xy for c in (x, y)), ln).reshape(-1, 2 * ln)
+
+
+def _unpack(out, ln, st=None, needs_host=False):
+    """The rows of an (n, ln) output as ints, of an (n, 2 ln) one as (x, y) pairs; None where `st` is not TRUE.
+    needs_host: refuse the batch if the engine flagged an input point as off the curve (ST_NEEDS_HOST)."""
+    if needs_host and bool((st == nat.ST_NEEDS_HOST).any()):
+        raise NeedsReferencePath("point %d is not on the curve; the reference does not validate it" % int(np.flatnonzero(st == nat.ST_NEEDS_HOST)[0]))
+    b = out.tobytes()
+    vals = [int.from_bytes(b[i:i + ln], "big") for i in range(0, len(b), ln)]
+    if out.shape[1] != ln:
+        vals = list(zip(vals[::2], vals[1::2]))
+    return [v if st is None or st[i] == nat.ST_TRUE else None for i, v in enumerate(vals)]
+
+
+def _blob(items):
+    """Byte strings back to back as a uint8 array, and the n + 1 uint64 offsets of the items in it."""
+    off = np.zeros(len(items) + 1, np.uint64)
+    off[1:] = np.cumsum([len(b) for b in items])
+    return np.frombuffer(b"".join(items), np.uint8), off
+
+
+def _answer(value, st, answers):
+    """One item's result: `value` where its status is one of `answers`, else the exception the reference throws."""
+    st = int(st)
+    if st not in answers:
+        raise EllipticError(_THROW_MSG.get(st, "status %d" % st))
+    return value
+
+
 def parse_der(data):
     """Signature._importDER (ec/signature.js:73-134).  Returns (r, s) or None."""
     n = len(data)
@@ -212,19 +281,6 @@ class EC:
             v -= self.n
         return v
 
-    def _signature(self, sig):
-        """new Signature(sig, 'hex') (ec/signature.js:8-22)."""
-        if isinstance(sig, dict):
-            if not (sig.get("r") and sig.get("s")):
-                raise EllipticError("Signature without r or s")
-            return _bn(sig["r"]), _bn(sig["s"])
-        if hasattr(sig, "r") and hasattr(sig, "s"):
-            return int(sig.r), int(sig.s)
-        rs = parse_der(_to_array(sig, "hex"))
-        if rs is None:
-            raise EllipticError("Signature without r or s")
-        return rs
-
     def _public(self, key, enc=None):
         """KeyPair._importPublic (ec/key.js:84-99) -> (fmt, bytes)."""
         ln = self._len
@@ -239,7 +295,7 @@ class EC:
             if x >> (8 * ln) or y >> (8 * ln):
                 x %= self._c["p"]
                 y %= self._c["p"]
-            return nat.PUB_XY, x.to_bytes(ln, "big") + y.to_bytes(ln, "big")
+            return nat.PUB_XY, _pack([x, y], ln).tobytes()
         b = _to_array(key, enc)
         if len(b) and b[0] in (4, 6, 7) and len(b) - 1 == 2 * ln:
             if (b[0] == 6 and b[-1] % 2 != 0) or (b[0] == 7 and b[-1] % 2 != 1):
@@ -249,25 +305,24 @@ class EC:
             return nat.PUB_SEC1_33, b
         raise EllipticError("Unknown point format")                # base.js:291
 
+    def _pub_bytes(self, pub_fmt):
+        """Bytes per public key in `pub_fmt` (include/elliptic_b200.h: EB200_PUB_*)."""
+        return {nat.PUB_XY: 2 * self._len, nat.PUB_SEC1_65: 1 + 2 * self._len, nat.PUB_SEC1_33: 1 + self._len}[pub_fmt]
+
     # ---- batch entry points ---------------------------------------------------
     def verify_batch_packed(self, e, r, s, pub, pub_fmt=nat.PUB_XY):
         """Packed form: e, r, s are (n, len) uint8 arrays (big-endian), pub is
         (n, 2*len).  Returns the per-item status bytes (see _native.ST_*)."""
         lib = nat.init(self._device)
-        e = np.ascontiguousarray(e, dtype=np.uint8)
-        r = np.ascontiguousarray(r, dtype=np.uint8)
-        s = np.ascontiguousarray(s, dtype=np.uint8)
-        pub = np.ascontiguousarray(pub, dtype=np.uint8)
+        e, r, s, pub = (np.ascontiguousarray(a, dtype=np.uint8) for a in (e, r, s, pub))
         n = e.shape[0]
         if not (e.shape == (n, self._len) and r.shape == e.shape and s.shape == e.shape):      # raw pointers go down
             raise ValueError("e, r, s must be (n, %d) uint8 arrays" % self._len)
-        pb = {nat.PUB_XY: 2 * self._len, nat.PUB_SEC1_65: 1 + 2 * self._len, nat.PUB_SEC1_33: 1 + self._len}[pub_fmt]
+        pb = self._pub_bytes(pub_fmt)
         if pub.shape != (n, pb):
             raise ValueError("pub must be (n, %d) for this format, got %r" % (pb, pub.shape))
         status = np.empty(n, dtype=np.uint8)
-        nat.check(lib.eb200_ecdsa_verify_batch(
-            self._c["id"], n, e.ctypes.data, r.ctypes.data, s.ctypes.data, pub.ctypes.data,
-            pub_fmt, status.ctypes.data))
+        nat.call(lib.eb200_ecdsa_verify_batch, self._c["id"], n, e, r, s, pub, pub_fmt, status)
         return status
 
     def verify_batch_der_packed(self, e, ders, pub, pub_fmt=nat.PUB_XY):
@@ -275,16 +330,13 @@ class EC:
         Signature._importDER, ec/signature.js:73-134); pub: (n, k) uint8 in `pub_fmt`.  Returns statuses."""
         lib = nat.init(self._device)
         n = len(ders)
-        off = np.zeros(n + 1, np.uint64)
-        off[1:] = np.cumsum([len(d) for d in ders])
-        blob = np.frombuffer(b"".join(bytes(d) for d in ders) + b"\x00", np.uint8)
+        blob, off = _blob([bytes(d) for d in ders])
         e = np.ascontiguousarray(e, np.uint8); pub = np.ascontiguousarray(pub, np.uint8)
-        pb = {nat.PUB_XY: 2 * self._len, nat.PUB_SEC1_65: 1 + 2 * self._len, nat.PUB_SEC1_33: 1 + self._len}[pub_fmt]
+        pb = self._pub_bytes(pub_fmt)
         if e.shape != (n, self._len) or pub.shape != (n, pb):
             raise EllipticError("verify_batch_der_packed: e must be (n, %d) and pub (n, %d)" % (self._len, pb))
         status = np.zeros(n, np.uint8)
-        nat.check(lib.eb200_ecdsa_verify_batch_der(self._c["id"], n, e.ctypes.data, blob.ctypes.data, off.ctypes.data,
-                                                   pub.ctypes.data, pub_fmt, status.ctypes.data))
+        nat.call(lib.eb200_ecdsa_verify_batch_der, self._c["id"], n, e, blob, off, pub, pub_fmt, status)
         return status
 
     def verify_batch(self, msgs, sigs, keys, enc=None, msg_bit_length=None):
@@ -292,30 +344,27 @@ class EC:
         Returns a uint8 array of statuses; items whose *parsing* throws in the
         reference raise here, like a loop over `verify` would at that item."""
         n = len(msgs)
-        ln = self._len
-        e = np.zeros((n, ln), np.uint8)
-        r = np.zeros((n, ln), np.uint8)
-        s = np.zeros((n, ln), np.uint8)
         groups = {}          # pub format -> (item indices, key bytes)
         early = {}
-        for i in range(n):
-            ev = self._truncate_to_n(msgs[i], msg_bit_length)
-            fmt, pb = self._public(keys[i], enc)
-            rv, sv = self._signature(sigs[i])
-            if rv < 1 or rv >= self.n or sv < 1 or sv >= self.n:
-                early[i] = nat.ST_FALSE       # ec/index.js:199-202 (after the key import, which may throw)
-                rv = sv = 0
-            e[i] = np.frombuffer(ev.to_bytes(ln, "big"), np.uint8)
-            r[i] = np.frombuffer(rv.to_bytes(ln, "big"), np.uint8)
-            s[i] = np.frombuffer(sv.to_bytes(ln, "big"), np.uint8)
-            g = groups.setdefault(fmt, ([], []))
-            g[0].append(i)
-            g[1].append(pb)
+
+        def items():         # parsed one item at a time, as _pack encodes them: an e that does not fit raises at its item
+            for i in range(n):
+                ev = self._truncate_to_n(msgs[i], msg_bit_length)
+                fmt, pb = self._public(keys[i], enc)
+                rv, sv = _signature(sigs[i], "hex")
+                if rv < 1 or rv >= self.n or sv < 1 or sv >= self.n:
+                    early[i] = nat.ST_FALSE       # ec/index.js:199-202 (after the key import, which may throw)
+                    rv = sv = 0
+                g = groups.setdefault(fmt, ([], []))
+                g[0].append(i)
+                g[1].append(pb)
+                yield from (ev, rv, sv)
+        ers = _pack(items(), self._len).reshape(n, 3, self._len)
         st = np.zeros(n, np.uint8)
         for fmt, (idx, pbs) in groups.items():
             idx = np.asarray(idx)
             pub = np.frombuffer(b"".join(pbs), np.uint8).reshape(len(pbs), -1)
-            st[idx] = self.verify_batch_packed(e[idx], r[idx], s[idx], pub, fmt)
+            st[idx] = self.verify_batch_packed(ers[idx, 0], ers[idx, 1], ers[idx, 2], pub, fmt)
         for i, v in early.items():
             if st[i] in (nat.ST_TRUE, nat.ST_FALSE, nat.ST_NEEDS_HOST):
                 st[i] = v
@@ -331,32 +380,30 @@ class EC:
             raise EllipticError("sign_batch: not available on " + self.name)
         lib = nat.init(self._device)
         n, ln = len(msgs), self._len
-        e = np.zeros((n, ln), np.uint8); d = np.zeros((n, ln), np.uint8)
+        es, ds = [], []
         for i in range(n):
             ev = self._truncate_to_n(msgs[i], msg_bit_length)                  # includes the single `- n` (ec/index.js:105-106)
             if ev >> (8 * ln):
                 raise EllipticError("byte array longer than desired length")   # msg.toArray('be', bytes), dist bn.js toArrayLike
-            e[i] = np.frombuffer(ev.to_bytes(ln, "big"), np.uint8)
-            d[i] = np.frombuffer((_bn(privs[i]) % self.n).to_bytes(ln, "big"), np.uint8)   # _importPrivate
+            es.append(ev)
+            ds.append(_bn(privs[i]) % self.n)                                  # _importPrivate
+        e, d = _pack(es, ln), _pack(ds, ln)
         r = np.zeros((n, ln), np.uint8); s = np.zeros((n, ln), np.uint8)
         rec = np.zeros(n, np.uint8); st = np.zeros(n, np.uint8)
         flags = 1 if canonical else 0
         if k is not None:
+            def nonce(i, it):
+                kv = _bn(k(int(i), it))
+                # _truncateToN(k, true) on a BN wider than the field: shift by its own byte length (ec/index.js:96-103)
+                delta = ((kv.bit_length() + 7) // 8) * 8 - self.n.bit_length()
+                return kv >> delta if kv.bit_length() > 8 * ln and delta > 0 else kv
             todo = np.arange(n)
             for it in range(1 << 16):
-                kb = np.zeros((len(todo), ln), np.uint8)
-                for j, i in enumerate(todo):
-                    kv = _bn(k(int(i), it))
-                    # _truncateToN(k, true) on a BN wider than the field: shift by its own byte length (ec/index.js:96-103)
-                    delta = ((kv.bit_length() + 7) // 8) * 8 - self.n.bit_length()
-                    if kv.bit_length() > 8 * ln and delta > 0:
-                        kv >>= delta
-                    kb[j] = np.frombuffer(kv.to_bytes(ln, "big"), np.uint8)
-                es, ds = np.ascontiguousarray(e[todo]), np.ascontiguousarray(d[todo])
+                kb = _pack((nonce(i, it) for i in todo), ln)     # k(i, it) is encoded before the next item's is asked for
                 rr = np.zeros((len(todo), ln), np.uint8); ss = np.zeros((len(todo), ln), np.uint8)
                 cc = np.zeros(len(todo), np.uint8); tt = np.zeros(len(todo), np.uint8)
-                nat.check(lib.eb200_ecdsa_sign_batch_k(self._c["id"], len(todo), es.ctypes.data, ds.ctypes.data, kb.ctypes.data, flags,
-                                                       rr.ctypes.data, ss.ctypes.data, cc.ctypes.data, tt.ctypes.data))
+                nat.call(lib.eb200_ecdsa_sign_batch_k, self._c["id"], len(todo), e[todo], d[todo], kb, flags,
+                         rr, ss, cc, tt)
                 ok = tt == nat.ST_TRUE
                 r[todo[ok]], s[todo[ok]], rec[todo[ok]], st[todo[ok]] = rr[ok], ss[ok], cc[ok], tt[ok]
                 if not bool(((tt == nat.ST_TRUE) | (tt == nat.ST_RETRY)).all()):
@@ -365,17 +412,14 @@ class EC:
                 if not len(todo):
                     break
         elif pers is not None:
-            pb = np.frombuffer(bytes(_to_array(pers, pers_enc or "utf8")) + b"\x00", np.uint8)
-            nat.check(lib.eb200_ecdsa_sign_batch_pers(self._c["id"], n, e.ctypes.data, d.ctypes.data, pb.ctypes.data, pb.size - 1, flags,
-                                                      r.ctypes.data, s.ctypes.data, rec.ctypes.data, st.ctypes.data))
+            pb, pb_len = _pers(pers, pers_enc)
+            nat.call(lib.eb200_ecdsa_sign_batch_pers, self._c["id"], n, e, d, pb, pb_len, flags, r, s, rec, st)
         else:
-            nat.check(lib.eb200_ecdsa_sign_batch(self._c["id"], n, e.ctypes.data, d.ctypes.data, flags,
-                                                 r.ctypes.data, s.ctypes.data, rec.ctypes.data, st.ctypes.data))
+            nat.call(lib.eb200_ecdsa_sign_batch, self._c["id"], n, e, d, flags, r, s, rec, st)
         if not bool((st == nat.ST_TRUE).all()):
             bad = int(np.flatnonzero(st != nat.ST_TRUE)[0])
             raise nat.NativeError("sign_batch: item %d returned status %d" % (bad, int(st[bad])))
-        return ([int.from_bytes(r[i].tobytes(), "big") for i in range(n)],
-                [int.from_bytes(s[i].tobytes(), "big") for i in range(n)], rec)
+        return _unpack(r, ln), _unpack(s, ln), rec
 
     def gen_key_pair_batch(self, entropies, entropy_enc=None, pers=None, pers_enc=None):
         """Batch of EC.prototype.genKeyPair({entropy, entropyEnc, pers, persEnc}) (ec/index.js:55-79): every item's key
@@ -393,15 +437,12 @@ class EC:
             raise EllipticError("Not enough entropy. Minimum is: 192 bits")     # hmac-drbg ctor, dist:8708-8710
         if any(len(x) != ne for x in ents):
             raise EllipticError("gen_key_pair_batch: entropies of one batch must have the same length")
-        eb = np.frombuffer(b"".join(ents), np.uint8).reshape(n, ne)
-        pb = np.frombuffer(bytes(_to_array(pers, pers_enc or "utf8")) + b"\x00", np.uint8) if pers is not None else None
+        pb, pb_len = _pers(pers, pers_enc)
         priv = np.zeros((n, ln), np.uint8); pub = np.zeros((n, 2 * ln), np.uint8); st = np.zeros(n, np.uint8)
-        nat.check(lib.eb200_ec_keygen_batch(self._c["id"], n, eb.ctypes.data, ne, pb.ctypes.data if pb is not None else None,
-                                            (pb.size - 1) if pb is not None else 0, priv.ctypes.data, pub.ctypes.data, st.ctypes.data))
+        nat.call(lib.eb200_ec_keygen_batch, self._c["id"], n, _blob(ents)[0], ne, pb, pb_len, priv, pub, st)
         if not bool((st == nat.ST_TRUE).all()):
             raise nat.NativeError("gen_key_pair_batch: unexpected status")
-        return ([int.from_bytes(priv[i].tobytes(), "big") for i in range(n)],
-                [(int.from_bytes(pub[i, :ln].tobytes(), "big"), int.from_bytes(pub[i, ln:].tobytes(), "big")) for i in range(n)])
+        return _unpack(priv, ln), _unpack(pub, ln)
 
     def sign(self, msg, priv, canonical=False, pers=None, pers_enc=None, k=None):
         """EC.prototype.sign (ec/index.js:110-186); k: the reference's options.k(iter)."""
@@ -409,6 +450,11 @@ class EC:
         return {"r": r[0], "s": s[0], "recoveryParam": int(rec[0])}
 
     # ---- public-key recovery -----------------------------------------------------------------------------
+    def _recover_args(self, es, rss):
+        """e mod n, r, s mod n as (n, len) arrays, as the recover and recovery-parameter entry points take them."""
+        ln = self._len
+        return _pack([e % self.n for e in es], ln), _pack([r for r, _ in rss], ln), _pack([s % self.n for _, s in rss], ln)
+
     def recover_pub_key_batch(self, msgs, sigs, js, enc=None):
         """Batch of EC.prototype.recoverPubKey (ec/index.js:231-259).  msgs as `new BN(msg)` takes them
         (int / hex / bytes, NOT truncated), sigs as Signature takes them, js the recovery params.
@@ -417,32 +463,24 @@ class EC:
             raise EllipticError("recover_pub_key_batch: short curves only")
         lib = nat.init(self._device)
         n, ln = len(msgs), self._len
-        e = np.zeros((n, ln), np.uint8); r = np.zeros((n, ln), np.uint8); s = np.zeros((n, ln), np.uint8)
-        rid = np.zeros(n, np.uint8)
+        es, rss, rid = [], [], []
         for i in range(n):
             if (3 & js[i]) != js[i]:
                 raise EllipticError("The recovery param is more than two bits")      # ec/index.js:232
-            rv, sv = self._signature_enc(sigs[i], enc)
-            ev = _bn(msgs[i]) if not isinstance(msgs[i], (bytes, bytearray, list, tuple)) else int.from_bytes(_to_array(msgs[i]), "big")
+            rv, sv = _signature(sigs[i], enc)
+            es.append(_msg_int(msgs[i]))
             if rv >> (8 * ln):
                 raise NeedsReferencePath("r does not fit the curve's field width")
-            e[i] = np.frombuffer((ev % self.n).to_bytes(ln, "big"), np.uint8)
-            r[i] = np.frombuffer(rv.to_bytes(ln, "big"), np.uint8)
-            s[i] = np.frombuffer((sv % self.n).to_bytes(ln, "big"), np.uint8)
-            rid[i] = js[i]
+            rss.append((rv, sv))
+            rid.append(js[i])
         out = np.zeros((n, 2 * ln), np.uint8)
         st = np.zeros(n, np.uint8)
-        nat.check(lib.eb200_ecdsa_recover_batch(self._c["id"], n, e.ctypes.data, r.ctypes.data, s.ctypes.data,
-                                                rid.ctypes.data, out.ctypes.data, st.ctypes.data))
-        pts = [(int.from_bytes(out[i, :ln].tobytes(), "big"), int.from_bytes(out[i, ln:].tobytes(), "big"))
-               if st[i] == nat.ST_TRUE else None for i in range(n)]
-        return pts, st
+        nat.call(lib.eb200_ecdsa_recover_batch, self._c["id"], n, *self._recover_args(es, rss), np.array(rid, np.uint8), out, st)
+        return _unpack(out, ln, st), st
 
     def recover_pub_key(self, msg, signature, j, enc=None):
         pts, st = self.recover_pub_key_batch([msg], [signature], [j], enc)
-        if st[0] in (nat.ST_TRUE, nat.ST_INFINITY):
-            return pts[0]
-        raise EllipticError(_THROW_MSG.get(int(st[0]), "status %d" % int(st[0])))
+        return _answer(pts[0], st[0], (nat.ST_TRUE, nat.ST_INFINITY))
 
     def get_key_recovery_param_batch(self, msgs, sigs, qs, enc=None):
         """Batch of EC.prototype.getKeyRecoveryParam (ec/index.js:261-278): per item the first j in 0..3 whose
@@ -457,9 +495,9 @@ class EC:
         js = [None] * n
         st = np.zeros(n, np.uint8)
         todo = []
-        rs = []
+        rss = []
         for i in range(n):
-            rv, sv = self._signature_enc(sigs[i], enc)                  # new Signature(signature, enc) may throw first
+            rv, sv = _signature(sigs[i], enc)                  # new Signature(signature, enc) may throw first
             rp = sigs[i].get("recoveryParam") if isinstance(sigs[i], dict) else \
                 getattr(sigs[i], "recoveryParam", getattr(sigs[i], "recovery_param", None))
             if rp is not None:
@@ -470,22 +508,15 @@ class EC:
             if rv >> (8 * ln):
                 raise NeedsReferencePath("r does not fit the curve's field width")
             todo.append(i)
-            rs.append((rv, sv))
+            rss.append((rv, sv))
         if not todo:
             return js, st
         lib = nat.init(self._device)
         m = len(todo)
-        e = np.zeros((m, ln), np.uint8); r = np.zeros((m, ln), np.uint8); s = np.zeros((m, ln), np.uint8)
-        for k, i in enumerate(todo):
-            rv, sv = rs[k]
-            ev = _bn(msgs[i]) if not isinstance(msgs[i], (bytes, bytearray, list, tuple)) else int.from_bytes(_to_array(msgs[i]), "big")
-            e[k] = np.frombuffer((ev % self.n).to_bytes(ln, "big"), np.uint8)
-            r[k] = np.frombuffer(rv.to_bytes(ln, "big"), np.uint8)
-            s[k] = np.frombuffer((sv % self.n).to_bytes(ln, "big"), np.uint8)
+        ers = self._recover_args([_msg_int(msgs[i]) for i in todo], rss)
         q = self._points([qs[i] for i in todo])
         rid = np.zeros(m, np.uint8); sub = np.zeros(m, np.uint8)
-        nat.check(lib.eb200_ecdsa_recovery_param_batch(self._c["id"], m, e.ctypes.data, r.ctypes.data, s.ctypes.data,
-                                                       q.ctypes.data, rid.ctypes.data, sub.ctypes.data))
+        nat.call(lib.eb200_ecdsa_recovery_param_batch, self._c["id"], m, *ers, q, rid, sub)
         for k, i in enumerate(todo):
             st[i] = sub[k]
             js[i] = int(rid[k]) if sub[k] == nat.ST_TRUE else None
@@ -494,32 +525,21 @@ class EC:
     def get_key_recovery_param(self, e, signature, Q, enc=None):
         """EC.prototype.getKeyRecoveryParam (ec/index.js:261-278): the parameter, or raises like the reference."""
         js, st = self.get_key_recovery_param_batch([e], [signature], [Q], enc)
-        if st[0] == nat.ST_TRUE:
-            return js[0]
-        raise EllipticError(_THROW_MSG.get(int(st[0]), "status %d" % int(st[0])))
+        return _answer(js[0], st[0], (nat.ST_TRUE,))
 
     # ---- curve.point(...).mul / mulAdd batches (short.js:422-441) ---------------------------------------------
     def _scalars(self, ks):
-        ln = self._len
-        out = np.zeros((len(ks), ln), np.uint8)
-        for i, k in enumerate(ks):
+        vals = []
+        for k in ks:
             k = _bn(k)
             if k < 0:
                 raise EllipticError("negative scalars are not supported by the batch path")
-            if k >> (8 * ln):
-                k %= self.n          # same point for every on-curve input
-            out[i] = np.frombuffer(k.to_bytes(ln, "big"), np.uint8)
-        return out
+            vals.append(k % self.n if k >> (8 * self._len) else k)          # same point for every on-curve input
+        return _pack(vals, self._len)
 
     def _points(self, pts):
         """curve.point(x, y) (short.js:251-271): coordinates reduced mod p, not validated."""
-        ln = self._len
-        out = np.zeros((len(pts), 2 * ln), np.uint8)
-        for i, pt in enumerate(pts):
-            x, y = (pt["x"], pt["y"]) if isinstance(pt, dict) else pt
-            out[i, :ln] = np.frombuffer((_bn(x) % self._c["p"]).to_bytes(ln, "big"), np.uint8)
-            out[i, ln:] = np.frombuffer((_bn(y) % self._c["p"]).to_bytes(ln, "big"), np.uint8)
-        return out
+        return _pack_points(pts, self._c["p"], self._len)
 
     def _mul_common(self, k1, k2, pts):
         if self.name == "curve25519":
@@ -531,15 +551,10 @@ class EC:
         out = np.zeros((n, 2 * ln), np.uint8)
         st = np.zeros(n, np.uint8)
         if k1 is None:
-            nat.check(lib.eb200_scalar_mul_batch(self._c["id"], n, k2.ctypes.data, pts.ctypes.data if pts is not None else None,
-                                                 out.ctypes.data, st.ctypes.data))
+            nat.call(lib.eb200_scalar_mul_batch, self._c["id"], n, k2, pts, out, st)
         else:
-            nat.check(lib.eb200_mul_add_batch(self._c["id"], n, k1.ctypes.data, k2.ctypes.data, pts.ctypes.data,
-                                              out.ctypes.data, st.ctypes.data))
-        if bool((st == nat.ST_NEEDS_HOST).any()):      # (only the Edwards preset reports it; the short curves replay)
-            raise NeedsReferencePath("point %d is not on the curve; the reference does not validate it" % int(np.flatnonzero(st == nat.ST_NEEDS_HOST)[0]))
-        return [(int.from_bytes(out[i, :ln].tobytes(), "big"), int.from_bytes(out[i, ln:].tobytes(), "big"))
-                if st[i] == nat.ST_TRUE else None for i in range(n)]
+            nat.call(lib.eb200_mul_add_batch, self._c["id"], n, k1, k2, pts, out, st)
+        return _unpack(out, ln, st, needs_host=True)      # (only the Edwards preset reports it; the short curves replay)
 
     def x_mul_batch(self, xs, ks):
         """curve25519: [curve.point(x).mul(k).getX()] (mont.js:130-153, 173-178) -- x-only points, no validation."""
@@ -547,16 +562,16 @@ class EC:
             raise EllipticError("x_mul_batch: curve25519 only")
         lib = nat.init(self._device)
         n = len(ks)
-        kb = np.zeros((n, 32), np.uint8); xb = np.zeros((n, 32), np.uint8)
+        kvs, xvs = [], []
         for i in range(n):
             kv, xv = _bn(ks[i]), _bn(xs[i])
             if kv >> 256:
                 raise NeedsReferencePath("scalar wider than 256 bits")
-            kb[i] = np.frombuffer(kv.to_bytes(32, "big"), np.uint8)
-            xb[i] = np.frombuffer((xv % self._c["p"] if xv >> 256 else xv).to_bytes(32, "big"), np.uint8)
+            kvs.append(kv)
+            xvs.append(xv % self._c["p"] if xv >> 256 else xv)
         out = np.zeros((n, 32), np.uint8); st = np.zeros(n, np.uint8)
-        nat.check(lib.eb200_x25519_mul_batch(n, kb.ctypes.data, xb.ctypes.data, out.ctypes.data, st.ctypes.data))
-        return [int.from_bytes(out[i].tobytes(), "big") for i in range(n)]
+        nat.call(lib.eb200_x25519_mul_batch, n, _pack(kvs, 32), _pack(xvs, 32), out, st)
+        return _unpack(out, 32)
 
     def g_mul_batch(self, ks):
         """[G.mul(k) for k in ks] (short.js:422-427, the keygen product ec/key.js:55-60): (x, y) or None = infinity."""
@@ -570,15 +585,6 @@ class EC:
         """[G.mulAdd(k1, P2, k2)] (short.js:434-441): (x, y) or None = infinity."""
         return self._mul_common(self._scalars(k1s), self._scalars(k2s), self._points(p2s))
 
-    def _signature_enc(self, sig, enc):
-        """new Signature(sig, enc) as recoverPubKey calls it (enc passed through, ec/index.js:233)."""
-        if isinstance(sig, dict) or (hasattr(sig, "r") and hasattr(sig, "s")):
-            return self._signature(sig)
-        rs = parse_der(_to_array(sig, enc))
-        if rs is None:
-            raise EllipticError("Signature without r or s")
-        return rs
-
     # ---- ECDH --------------------------------------------------------------------------------------------
     def derive_batch(self, privs, pubs):
         """Batch of `ec.keyFromPrivate(priv).derive(ec.keyFromPublic(pub).getPublic())`
@@ -588,20 +594,15 @@ class EC:
             return self._derive_short(privs, pubs)
         lib = nat.init(self._device)
         n = len(privs)
-        k = np.zeros((n, 32), np.uint8)
-        x = np.zeros((n, 32), np.uint8)
+        kvs, xvs = [], []
         for i in range(n):
-            kv = _bn(privs[i]) % self.n                      # _importPrivate: umod n
+            kvs.append(_bn(privs[i]) % self.n)                      # _importPrivate: umod n
             xv = _bn(pubs[i])
-            if xv >> 256:
-                xv %= self._c["p"]
-            k[i] = np.frombuffer(kv.to_bytes(32, "big"), np.uint8)
-            x[i] = np.frombuffer(xv.to_bytes(32, "big"), np.uint8)
+            xvs.append(xv % self._c["p"] if xv >> 256 else xv)
         out = np.zeros((n, 32), np.uint8)
         st = np.zeros(n, np.uint8)
-        nat.check(lib.eb200_x25519_derive_batch(n, k.ctypes.data, x.ctypes.data, out.ctypes.data, st.ctypes.data))
-        vals = [int.from_bytes(out[i].tobytes(), "big") if st[i] == nat.ST_TRUE else None for i in range(n)]
-        return vals, st
+        nat.call(lib.eb200_x25519_derive_batch, n, _pack(kvs, 32), _pack(xvs, 32), out, st)
+        return _unpack(out, 32, st), st
 
     def derive_batch_packed(self, priv, pubx, out=None, status=None):
         """Packed curve25519 ECDH: priv, pubx are (n, 32) uint8 arrays (big-endian; priv already reduced mod n as
@@ -619,7 +620,7 @@ class EC:
         st = np.empty(n, np.uint8) if status is None else status
         if out.shape != (n, 32) or out.dtype != np.uint8 or not out.flags.c_contiguous or st.shape != (n,) or st.dtype != np.uint8:
             raise EllipticError("derive_batch_packed: out must be a contiguous (n, 32) uint8 array, status (n,) uint8")
-        nat.check(lib.eb200_x25519_derive_batch(n, priv.ctypes.data, pubx.ctypes.data, out.ctypes.data, st.ctypes.data))
+        nat.call(lib.eb200_x25519_derive_batch, n, priv, pubx, out, st)
         return out, st
 
     def _derive_short(self, privs, pubs):
@@ -630,25 +631,18 @@ class EC:
         pts = self._points(pubs)
         out = np.zeros((n, ln), np.uint8)
         st = np.zeros(n, np.uint8)
-        nat.check(lib.eb200_ecdh_derive_batch(self._c["id"], n, k.ctypes.data, pts.ctypes.data, out.ctypes.data, st.ctypes.data))
-        vals = [int.from_bytes(out[i].tobytes(), "big") if st[i] == nat.ST_TRUE else None for i in range(n)]
-        return vals, st
+        nat.call(lib.eb200_ecdh_derive_batch, self._c["id"], n, k, pts, out, st)
+        return _unpack(out, ln, st), st
 
     def derive(self, priv, pub):
         """KeyPair.prototype.derive: the shared x as an int, or raises like the reference."""
         vals, st = self.derive_batch([priv], [pub])
-        if st[0] == nat.ST_TRUE:
-            return vals[0]
-        raise EllipticError(_THROW_MSG.get(int(st[0]), "status %d" % int(st[0])))
+        return _answer(vals[0], st[0], (nat.ST_TRUE,))
 
     def verify(self, msg, signature, key, enc=None, options=None):
         """EC.prototype.verify (ec/index.js:188-229): bool, or raises."""
         mbl = (options or {}).get("msgBitLength")
         st = int(self.verify_batch([msg], [signature], [key], enc, mbl)[0])
-        if st == nat.ST_TRUE:
-            return True
-        if st == nat.ST_FALSE:
-            return False
         if st == nat.ST_NEEDS_HOST:
             raise NeedsReferencePath("public key is not on the curve; the reference does not validate it")
-        raise EllipticError(_THROW_MSG.get(st, "status %d" % st))
+        return _answer(st == nat.ST_TRUE, st, (nat.ST_TRUE, nat.ST_FALSE))

@@ -11,7 +11,7 @@ import hashlib
 import numpy as np
 
 from . import _native as nat
-from .ec import EllipticError, _to_array, _THROW_MSG
+from .ec import EllipticError, _answer, _blob, _pack, _to_array
 
 N_ED25519 = 0x1000000000000000000000000000000014DEF9DEA2F79CD65812631A5CF5D3ED
 
@@ -44,8 +44,7 @@ class EDDSA:
         if not (R.shape == (n, 32) and S.shape == R.shape and A.shape == R.shape and h.shape == R.shape):
             raise ValueError("R, S, A, h must be (n, 32) uint8 arrays")
         status = np.empty(n, np.uint8)
-        nat.check(lib.eb200_eddsa_verify_batch(n, R.ctypes.data, S.ctypes.data, A.ctypes.data, h.ctypes.data,
-                                               status.ctypes.data))
+        nat.call(lib.eb200_eddsa_verify_batch, n, R, S, A, h, status)
         return status
 
     def verify_batch_msgs_packed(self, R, S, A, msgs, msg_off):
@@ -61,37 +60,17 @@ class EDDSA:
         if not (msg_off.shape == (n + 1,) and int(msg_off[n]) == msgs.size):
             raise ValueError("msg_off must hold n + 1 offsets, the last one equal to len(msgs)")
         status = np.empty(n, np.uint8)
-        nat.check(lib.eb200_eddsa_verify_batch_msgs(n, R.ctypes.data, S.ctypes.data, A.ctypes.data,
-                                                    msgs.ctypes.data if msgs.size else None, msg_off.ctypes.data,
-                                                    status.ctypes.data))
+        nat.call(lib.eb200_eddsa_verify_batch_msgs, n, R, S, A, msgs if msgs.size else None, msg_off, status)
         return status
 
     def verify_batch(self, messages, sigs, pubs, gpu_hash=True):
         """EDDSA#verifyBatch: lists of the reference's own argument forms (hex strings / byte arrays).
         gpu_hash=False computes hashInt with hashlib on the host instead of on the GPU."""
         n = len(messages)
-        R = np.zeros((n, 32), np.uint8)
-        S = np.zeros((n, 32), np.uint8)
-        A = np.zeros((n, 32), np.uint8)
-        h = np.zeros((n, 32), np.uint8)
-        if gpu_hash:
-            ms = []
-            for i in range(n):
-                sig = _parse_bytes(sigs[i])
-                if len(sig) != 2 * self.encoding_length:
-                    raise EllipticError("Signature has invalid size")   # eddsa/signature.js:23-24
-                pub = _parse_bytes(pubs[i])
-                if len(pub) != self.encoding_length:
-                    raise EllipticError("unsupported public key length %d" % len(pub))
-                R[i] = np.frombuffer(sig[:32], np.uint8)
-                S[i] = np.frombuffer(sig[32:], np.uint8)
-                A[i] = np.frombuffer(pub, np.uint8)
-                ms.append(_parse_bytes(messages[i]))
-            off = np.zeros(n + 1, np.uint64)
-            off[1:] = np.cumsum([len(m) for m in ms])
-            return self.verify_batch_msgs_packed(R, S, A, np.frombuffer(b"".join(ms), np.uint8), off)
+        rsa, ms = [], []
         for i in range(n):
-            msg = _parse_bytes(messages[i])
+            if not gpu_hash:
+                ms.append(_parse_bytes(messages[i]))      # the host path reads the message first
             sig = _parse_bytes(sigs[i])
             if len(sig) != 2 * self.encoding_length:
                 raise EllipticError("Signature has invalid size")       # eddsa/signature.js:23-24
@@ -99,11 +78,14 @@ class EDDSA:
             if len(pub) != self.encoding_length:
                 # decodePoint on another length reads a different y; not on the accelerated path
                 raise EllipticError("unsupported public key length %d" % len(pub))
-            R[i] = np.frombuffer(sig[:32], np.uint8)
-            S[i] = np.frombuffer(sig[32:], np.uint8)
-            A[i] = np.frombuffer(pub, np.uint8)
-            h[i] = np.frombuffer(self.hash_int(sig[:32], pub, msg).to_bytes(32, "little"), np.uint8)
-        return self.verify_batch_packed(R, S, A, h)
+            rsa.append(sig + pub)
+            if gpu_hash:
+                ms.append(_parse_bytes(messages[i]))
+        rows = _blob(rsa)[0].reshape(n, 96)
+        R, S, A = rows[:, :32], rows[:, 32:64], rows[:, 64:]
+        if gpu_hash:
+            return self.verify_batch_msgs_packed(R, S, A, *_blob(ms))
+        return self.verify_batch_packed(R, S, A, _pack([self.hash_int(x[:32], x[64:], m) for x, m in zip(rsa, ms)], 32, "little"))
 
     def sign_batch_packed(self, secrets, msgs, msg_off, want_pub=False):
         """secrets: (n, 32) uint8; msgs: concatenated message bytes; msg_off: n + 1 uint64 offsets.
@@ -118,8 +100,7 @@ class EDDSA:
         sig = np.empty((n, 64), np.uint8)
         pub = np.empty((n, 32), np.uint8) if want_pub else None
         st = np.empty(n, np.uint8)
-        nat.check(lib.eb200_eddsa_sign_batch(n, secrets.ctypes.data, msgs.ctypes.data if msgs.size else None, msg_off.ctypes.data,
-                                             sig.ctypes.data, pub.ctypes.data if want_pub else None, st.ctypes.data))
+        nat.call(lib.eb200_eddsa_sign_batch, n, secrets, msgs if msgs.size else None, msg_off, sig, pub, st)
         if not bool((st == nat.ST_TRUE).all()):
             raise nat.NativeError("eddsa sign: unexpected status")
         return (sig, pub) if want_pub else sig
@@ -128,17 +109,14 @@ class EDDSA:
         """EDDSA#signBatch: lists of the reference's own argument forms (hex strings / byte arrays); secrets as
         eddsa.keyFromSecret takes them.  Returns a list of 64-byte signatures (sig.toBytes())."""
         n = len(messages)
-        sec = np.zeros((n, 32), np.uint8)
-        ms = []
+        sks, ms = [], []
         for i in range(n):
             sk = _parse_bytes(secrets[i])
             if len(sk) != 32:
                 raise EllipticError("unsupported secret length %d" % len(sk))
-            sec[i] = np.frombuffer(bytes(sk), np.uint8)
-            ms.append(bytes(_parse_bytes(messages[i])))
-        off = np.zeros(n + 1, np.uint64)
-        off[1:] = np.cumsum([len(m) for m in ms])
-        sig = self.sign_batch_packed(sec, np.frombuffer(b"".join(ms), np.uint8), off)
+            sks.append(sk)
+            ms.append(_parse_bytes(messages[i]))
+        sig = self.sign_batch_packed(_blob(sks)[0].reshape(n, 32), *_blob(ms))
         return [sig[i].tobytes() for i in range(n)]
 
     def sign(self, message, secret):
@@ -155,8 +133,4 @@ class EDDSA:
     def verify(self, message, sig, pub):
         """EDDSA.prototype.verify (eddsa/index.js:52-63): bool, or raises."""
         st = int(self.verify_batch([message], [sig], [pub])[0])
-        if st == nat.ST_TRUE:
-            return True
-        if st == nat.ST_FALSE:
-            return False
-        raise EllipticError(_THROW_MSG.get(st, "status %d" % st))
+        return _answer(st == nat.ST_TRUE, st, (nat.ST_TRUE, nat.ST_FALSE))
