@@ -325,6 +325,63 @@ static napi_value X25519Batch(napi_env env, napi_callback_info info) {
   return res;
 }
 
+/* Key sets (eb200_keyset_*): the handle travels as an external whose box is shared with the finalizer, so that
+ * keysetDestroy and garbage collection free the set exactly once.
+ * keysetCreate(curveId, pub, pubFmt, tableBits) -> {handle, status: Uint8Array(m), tableBits, deviceBytes} */
+typedef struct { eb200_keyset* ks; } keyset_box;
+static void keyset_finalize(napi_env env, void* data, void* hint) {
+  (void)env; (void)hint;
+  keyset_box* b = (keyset_box*)data;
+  eb200_keyset_destroy(b->ks);
+  free(b);
+}
+static napi_value KeysetCreate(napi_env env, napi_callback_info info) {
+  ARGS(4); I32(0, curve); BUF(1, pub, lp); U32(2, fmt); U32(3, bits);
+  size_t len = field_len(curve), pb = pub_bytes(len, fmt);
+  if (!len || !pb) return fail(env, EB200_ERR_UNSUPPORTED);
+  size_t m = lp / pb;
+  if (lp != m * pb) return fail(env, EB200_ERR_ARG);
+  keyset_box* b = (keyset_box*)calloc(1, sizeof *b);
+  if (!b) return fail(env, EB200_ERR_ARG);
+  uint8_t* st; napi_value arr = out_u8(env, m, &st);
+  int rc = eb200_keyset_create(curve, m, pub, fmt, bits, st, &b->ks);
+  if (rc) { free(b); return fail(env, rc); }
+  uint32_t w = 0; size_t bytes = 0;
+  eb200_keyset_info(b->ks, 0, 0, &w, &bytes);
+  napi_value o = obj(env), h, vw, vb;
+  napi_create_external(env, b, keyset_finalize, 0, &h);
+  napi_create_uint32(env, w, &vw);
+  napi_create_double(env, (double)bytes, &vb);
+  SET(o, "handle", h); SET(o, "status", arr); SET(o, "tableBits", vw); SET(o, "deviceBytes", vb);
+  return o;
+}
+/* keysetDestroy(handle): frees the set now; the handle stays valid and answers EB200_ERR_ARG afterwards */
+static napi_value KeysetDestroy(napi_env env, napi_callback_info info) {
+  ARGS(1);
+  void* p = 0; napi_value undef;
+  if (napi_get_value_external(env, argv[0], &p) != napi_ok || !p) return fail(env, EB200_ERR_ARG);
+  keyset_box* b = (keyset_box*)p;
+  int rc = eb200_keyset_destroy(b->ks);
+  b->ks = 0;
+  if (rc) return fail(env, rc);
+  napi_get_undefined(env, &undef);
+  return undef;
+}
+/* ecdsaVerifyBatchKeyed(handle, e, r, s, keyIdx: Uint8Array over n little-endian uint32) -> Uint8Array(n) of statuses */
+static napi_value EcdsaVerifyBatchKeyed(napi_env env, napi_callback_info info) {
+  ARGS(5); BUF(1, e, le); BUF(2, r, lr); BUF(3, s, ls); BUF(4, idx, li);
+  void* p = 0;
+  if (napi_get_value_external(env, argv[0], &p) != napi_ok || !p || !((keyset_box*)p)->ks) return fail(env, EB200_ERR_ARG);
+  eb200_keyset* ks = ((keyset_box*)p)->ks;
+  int curve = 0;
+  eb200_keyset_info(ks, &curve, 0, 0, 0);
+  size_t len = field_len(curve), n = li / 4;
+  if (!len || li != 4 * n || le != n * len || lr != le || ls != le || ((uintptr_t)idx & 3)) return fail(env, EB200_ERR_ARG);
+  uint8_t* st; napi_value arr = out_u8(env, n, &st);
+  int rc = eb200_ecdsa_verify_batch_keyed(ks, n, e, r, s, (const uint32_t*)(const void*)idx, st);
+  return rc ? fail(env, rc) : arr;
+}
+
 static napi_value Register(napi_env env, napi_value exports) {
   static const struct { const char* name; napi_callback cb; } fns[] = {
       {"init", Init}, {"ecdsaVerifyBatch", EcdsaVerifyBatch}, {"ecdsaVerifyBatchAsync", EcdsaVerifyBatchAsync},
@@ -332,7 +389,8 @@ static napi_value Register(napi_env env, napi_value exports) {
       {"ecdsaRecoverBatch", EcdsaRecoverBatch}, {"ecdsaRecoveryParamBatch", EcdsaRecoveryParamBatch},
       {"mulAddBatch", MulAddBatch}, {"ecdhDeriveBatch", EcdhDeriveBatch},
       {"curveOpBatch", CurveOpBatch}, {"eddsaVerifyBatch", EddsaVerifyBatch}, {"eddsaSignBatch", EddsaSignBatch},
-      {"x25519Batch", X25519Batch}};
+      {"x25519Batch", X25519Batch},
+      {"keysetCreate", KeysetCreate}, {"keysetDestroy", KeysetDestroy}, {"ecdsaVerifyBatchKeyed", EcdsaVerifyBatchKeyed}};
   for (unsigned i = 0; i < sizeof fns / sizeof fns[0]; i++) {
     napi_value f;
     napi_create_function(env, fns[i].name, NAPI_AUTO_LENGTH, fns[i].cb, 0, &f);

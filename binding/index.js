@@ -97,6 +97,37 @@ elliptic.ec.prototype.verifyBatchWire = function verifyBatchWire(hashes, ders, k
   return Array.prototype.map.call(st, function(v, i) { return v === 4 ? self.verify(hashes[i], ders[i], keys[i]) : statusToBool(v); });
 };
 
+// EC#keySet(pubs[, enc]) -> {status, tableBits, deviceBytes, verifyBatch(msgs, sigs, keyIdx[, options]), destroy()}: the
+// batch form of `key = ec.keyFromPublic(pub, enc); key.getPublic().precompute()` once and key.verify(msg, sig) many times.
+// The keys are imported here (a key that throws, throws here, as keyFromPublic does) and kept on the GPU with their tables.
+elliptic.ec.prototype.keySet = function keySet(pubs, enc) {
+  var id = curveId(this), self = this, len = this.curve.p.byteLength();
+  if (id === undefined || this.curve.type !== 'short') throw new Error('key sets: short preset curves only');
+  init();
+  var keys = pubs.map(function(k) { return self.keyFromPublic(k, enc); });
+  var xy = pack(keys, 2 * len, function(k) { var P = k.getPublic(); return be(P.getX(), len).concat(be(P.getY(), len)); });
+  var set = native.keysetCreate(id, xy, 0, 0);
+  var Signature = this.sign('00', '01').constructor;
+  return {
+    status: set.status, tableBits: set.tableBits, deviceBytes: set.deviceBytes,
+    verifyBatch: function(msgs, sigs, keyIdx, options) {
+      var n = msgs.length, e = new Uint8Array(n * len), r = new Uint8Array(n * len), s = new Uint8Array(n * len), early = {};
+      var idx = new Uint32Array(n);
+      for (var i = 0; i < n; i++) {
+        if (!(keyIdx[i] >= 0 && keyIdx[i] < keys.length)) throw new Error('key index out of range');
+        idx[i] = keyIdx[i];
+        var msg = self._truncateToN(msgs[i], false, options && options.msgBitLength);
+        var sig = new Signature(sigs[i], 'hex');
+        if (sig.r.cmpn(1) < 0 || sig.r.cmp(self.n) >= 0 || sig.s.cmpn(1) < 0 || sig.s.cmp(self.n) >= 0) { early[i] = false; continue; }
+        e.set(be(msg, len), i * len); r.set(be(sig.r, len), i * len); s.set(be(sig.s, len), i * len);
+      }
+      var st = native.ecdsaVerifyBatchKeyed(set.handle, e, r, s, new Uint8Array(idx.buffer));
+      return Array.prototype.map.call(st, function(v, i) { return i in early ? false : statusToBool(v); });
+    },
+    destroy: function() { native.keysetDestroy(set.handle); }
+  };
+};
+
 // EC#signBatch(msgs, keys[, enc][, options]) -> Array<Signature>.  options: canonical, pers / persEnc (one string for the
 // batch), k: function(item, iter) -> BN (the reference's options.k per item), msgBitLength.
 elliptic.ec.prototype.signBatch = function signBatch(msgs, keys, enc, options) {

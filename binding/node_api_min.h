@@ -38,6 +38,11 @@ napi_status napi_get_value_int32(napi_env env, napi_value value, int32_t* result
 napi_status napi_create_arraybuffer(napi_env env, size_t byte_length, void** data, napi_value* result);
 napi_status napi_create_typedarray(napi_env env, napi_typedarray_type type, size_t length, napi_value arraybuffer, size_t byte_offset, napi_value* result);
 napi_status napi_create_object(napi_env env, napi_value* result);
+typedef void (*napi_finalize)(napi_env env, void* finalize_data, void* finalize_hint);
+napi_status napi_create_external(napi_env env, void* data, napi_finalize finalize_cb, void* finalize_hint, napi_value* result);
+napi_status napi_get_value_external(napi_env env, napi_value value, void** result);
+napi_status napi_create_uint32(napi_env env, uint32_t value, napi_value* result);
+napi_status napi_create_double(napi_env env, double value, napi_value* result);
 napi_status napi_create_function(napi_env env, const char* utf8name, size_t length, napi_callback cb, void* data, napi_value* result);
 napi_status napi_set_named_property(napi_env env, napi_value object, const char* utf8name, napi_value value);
 napi_status napi_throw_error(napi_env env, const char* code, const char* msg);

@@ -18,6 +18,7 @@ ST_FALSE, ST_TRUE, ST_THROW_INVALID_POINT, ST_THROW_NOT_VALIDATED, ST_NEEDS_HOST
 ST_INFINITY, ST_THROW_SECOND_KEY, ST_THROW_SIG_FORMAT, ST_RETRY, ST_THROW_NO_RECOVERY = 7, 8, 9, 10, 11
 CURVE_SECP256K1, CURVE_P256, CURVE_P384, CURVE_ED25519, CURVE_CURVE25519, CURVE_P521, CURVE_P192, CURVE_P224 = 1, 2, 3, 4, 5, 6, 7, 8
 PUB_XY, PUB_SEC1_65, PUB_SEC1_33 = 0, 1, 2
+KEYSET_MIN_BITS, KEYSET_MAX_BITS, KEYSET_DEFAULT_BUDGET = 4, 8, 1 << 30
 
 EXPORTS = [
     "eb200_init", "eb200_shutdown", "eb200_device_count", "eb200_strerror", "eb200_last_error", "eb200_last_timing",
@@ -30,6 +31,7 @@ EXPORTS = [
     "eb200_ecdsa_sign_batch_k", "eb200_ecdsa_sign_batch_pers", "eb200_ec_keygen_batch", "eb200_x25519_mul_batch",
     "eb200_curve_mul_batch", "eb200_curve_mul_add_batch", "eb200_curve_add_batch", "eb200_curve_dbl_batch", "eb200_curve_validate_batch",
     "eb200_ecdsa_recovery_param_batch",
+    "eb200_keyset_create", "eb200_keyset_info", "eb200_keyset_destroy", "eb200_ecdsa_verify_batch_keyed",
 ]
 
 
@@ -95,6 +97,10 @@ def load():
     lib.eb200_ecdsa_sign_batch.argtypes = [c.c_int, c.c_size_t, c.c_void_p, c.c_void_p, c.c_uint32] + [c.c_void_p] * 4
     lib.eb200_ecdsa_recover_batch.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 6
     lib.eb200_ecdsa_recovery_param_batch.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 6
+    lib.eb200_keyset_create.argtypes = [c.c_int, c.c_size_t, c.c_void_p, c.c_uint32, c.c_uint32, c.c_void_p, c.POINTER(c.c_void_p)]
+    lib.eb200_keyset_info.argtypes = [c.c_void_p, c.POINTER(c.c_int), c.POINTER(c.c_size_t), c.POINTER(c.c_uint32), c.POINTER(c.c_size_t)]
+    lib.eb200_keyset_destroy.argtypes = [c.c_void_p]
+    lib.eb200_ecdsa_verify_batch_keyed.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 5
     lib.eb200_ecdsa_verify_batch_der.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 4 + [c.c_uint32, c.c_void_p]
     lib.eb200_ecdh_derive_batch.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 4
     lib.eb200_scalar_mul_batch.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 4

@@ -26,6 +26,7 @@
 #include "sw_runtime.cuh"
 #include "kernel_bounds.h"
 #include "recovery_param.h"
+#include "keyset.h"
 
 using namespace eb;
 
@@ -948,14 +949,12 @@ void merge_timing(eb200_timing& a, const eb200_timing& b) {
   a.launches += b.launches;
 }
 
-// Runs fn(ctx, lo, m) over contiguous blocks of [0, n): one block per initialised device when the batch is
+// Runs fn(ctx, lo, m) over contiguous blocks of [0, n): one block per listed device (run_sharded: per initialised device) when the batch is
 // large enough, each on its own host thread (the blocks never exchange data; results land in the caller's
 // buffers at their own offsets).  A single-block call rotates over the devices so that concurrent callers
 // spread out.  Timing: the slowest block, launches summed.
 template <class F>
-int run_sharded(size_t n, F&& fn) {
-  int devs[MAX_DEV], nd;
-  { std::lock_guard<std::mutex> lk(g_mu); nd = g_ndev; for (int i = 0; i < nd; i++) devs[i] = g_devs[i]; }
+int run_sharded_on(const int* devs, int nd, size_t n, F&& fn) {
   if (nd == 0) return EB200_ERR_NOT_INIT;
   int use = (int)(n / SHARD_MIN_ITEMS);
   if (use > nd) use = nd;
@@ -999,6 +998,13 @@ int run_sharded(size_t n, F&& fn) {
   }
   t_timing = tm;
   return rc;
+}
+
+template <class F>
+int run_sharded(size_t n, F&& fn) {
+  int devs[MAX_DEV], nd;
+  { std::lock_guard<std::mutex> lk(g_mu); nd = g_ndev; for (int i = 0; i < nd; i++) devs[i] = g_devs[i]; }
+  return run_sharded_on(devs, nd, n, fn);
 }
 
 // A device -> host copy; rows > 1: `rows` rows of `bytes`, `pitch` bytes apart on the device, packed on the host.
@@ -1112,6 +1118,8 @@ int run_dev(const void* d_status, int table_curve, void* stream, Run&& run) {
 }
 }  // namespace
 
+static void keysets_release_all();     // key sets (end of this file): eb200_shutdown frees their device memory
+
 extern "C" {
 
 const char* eb200_strerror(int code) {
@@ -1163,6 +1171,7 @@ int eb200_init(const int* devices, int ndev, uint32_t flags) {
 
 int eb200_shutdown(void) {
   std::lock_guard<std::mutex> lk(g_mu);
+  keysets_release_all();
   for (int i = 0; i < g_ndev; i++) {
     Ctx& c = g_ctx[g_devs[i]];
     std::lock_guard<std::mutex> lc(c.mu);
@@ -1989,6 +1998,212 @@ int eb200_ecdsa_recovery_param_batch(int curve, size_t n, const uint8_t* e, cons
   return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
     return recovery_param_on(c, curve, m, e + lo * len, r + lo * len, s + lo * len, q_xy + lo * 2 * len, out_recid + lo,
                              status + lo);
+  });
+}
+
+}  // extern "C"
+
+// ---- key sets ---------------------------------------------------------------------------------------------------------
+// The kernels are in keyset.cu (see there why); this side owns the handles, stages the buffers and launches the unchanged
+// decode and prep kernels of this file around them.
+struct eb200_keyset {
+  int curve = 0;
+  size_t m = 0;
+  u32 W = 0, fmt = 0;
+  size_t device_bytes = 0;
+  bool live = false;                  // false once eb200_shutdown has freed the device copies
+  int ndev = 0;
+  int devs[MAX_DEV] = {};             // the devices that hold a copy: keyed calls are sharded over these only
+  KeysetDev dev[MAX_DEV] = {};        // indexed by CUDA ordinal, like g_ctx
+};
+
+namespace {
+std::mutex g_ks_mu;                   // the list of live sets (taken inside g_mu by shutdown, never the other way round)
+std::vector<eb200_keyset*> g_keysets;
+
+// frees the device copies; the caller holds whatever keeps the set's devices from being used
+void keyset_free_device(eb200_keyset* ks) {
+  for (int i = 0; i < ks->ndev; i++) {
+    KeysetDev& d = ks->dev[ks->devs[i]];
+    if (cudaSetDevice(ks->devs[i]) != cudaSuccess) { cudaGetLastError(); continue; }
+    cudaFree(d.xy); cudaFree(d.kst); cudaFree(d.tab);
+    d = KeysetDev{};
+  }
+  ks->ndev = 0;
+  ks->live = false;
+}
+
+// One device's copy of the set: keys up, decode (this file's kernels), classify + tables (keyset.cu), verdicts home.
+int keyset_build_on(Ctx& c, eb200_keyset* ks, const uint8_t* pub, uint8_t* key_status) {
+  const int curve = ks->curve;
+  const size_t m = ks->m, len = curve_len(curve), pb = pub_item_bytes(len, ks->fmt);
+  const int windows = keyset_windows(curve, (int)ks->W);
+  int rc = ensure_table(c, curve);
+  if (rc) return rc;
+  KeysetDev& d = ks->dev[c.device];
+  d.W = (int)ks->W;
+  CK(cudaMalloc(&d.xy, 2 * len * m));
+  CK(cudaMalloc(&d.kst, m));
+  CK(cudaMalloc(&d.tab, keyset_key_bytes(curve, (int)ks->W) * m));
+  if ((rc = grow(&c.d_in, &c.d_in_cap, align256(m * pb) + m))) return rc;
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, m * windows * 3 * keyset_geom(curve).limbs * 4))) return rc;
+  uint8_t *d_pub = c.d_in, *d_pre = c.d_in + align256(m * pb);
+  return run_single(c, {{d_pub, pub, m * pb}},
+    [&](Launch& L) {
+      const uint8_t* pre = nullptr;
+      if (ks->fmt == EB200_PUB_XY) CK(cudaMemcpyAsync(d.xy, d_pub, 2 * len * m, cudaMemcpyDeviceToDevice, L.st));
+      else {
+        pre = d_pre;
+        int rc2 = with_curve(curve, [&](auto cv) {
+          typedef decltype(cv) T;
+          if constexpr (is_k256<T>) L(k256_decode_pub_kernel, blocks128(m), 128, m, d_pub, ks->fmt, d.xy, d_pre);
+          else if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;
+          else L(sw_decode_pub_kernel<typename T::C>, blocks128(m), 128, m, d_pub, ks->fmt, d.xy, d_pre);
+          return L.rc;
+        });
+        if (rc2) return rc2;
+      }
+      cudaError_t err = keyset_build_launch(curve, m, d, pre, (u32*)c.d_ws, L.st, &L.count);
+      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_build_launch");
+    },
+    {{key_status, d.kst, m}}, {}, true);
+}
+
+// Keyed verify of one block on one device of the set, chunked like verify_on.
+int verify_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
+                    const u32* key_idx, uint8_t* status) {
+  const int curve = ks->curve;
+  const KeysetDev& d = ks->dev[c.device];
+  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
+  int rc = ensure_table(c, curve);
+  if (rc) return rc;
+  const size_t len = curve_len(curve);
+  const ChunkPlan P = make_plan(n);
+  const size_t idx_bytes = align256(n * 4);
+  if ((rc = grow(&c.d_in, &c.d_in_cap, idx_bytes + align256(n * 3 * len) + 1024))) return rc;
+  const WsLayout W = ws_layout(curve, P.max_m);
+  const size_t ws_slot = W.qtab;                    // prep words and the inversion scratch; no per-item table
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, (P.chunks > 1 ? 2 : 1) * ws_slot))) return rc;
+  if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
+  u32* d_idx = (u32*)c.d_in;
+  uint8_t *d_e = c.d_in + idx_bytes, *d_r = d_e + n * len, *d_s = d_r + n * len;
+  return run_chunked(c, P,
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {d_e + lo * len, e + lo * len, m * len};
+      seg[1] = {d_r + lo * len, r + lo * len, m * len};
+      seg[2] = {d_s + lo * len, s + lo * len, m * len};
+      seg[3] = {d_idx + lo, key_idx + lo, m * 4};
+      return 4;
+    },
+    [&](size_t lo, size_t m, Launch& L, int slot, int k) {
+      u32* ws = (u32*)(c.d_ws + (size_t)slot * ws_slot + W.ws);
+      u32* scratch = (u32*)(c.d_ws + (size_t)slot * ws_slot + W.scratch);
+      const u32* replay = nullptr;
+      int rc2 = with_curve(curve, [&](auto cv) {
+        typedef decltype(cv) T;
+        if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;
+        else if constexpr (is_k256<T>) {
+          L(k256_prep_kernel, batch_blocks(m, PREP_BATCH), 128, m, d_e + lo * len, d_r + lo * len, d_s + lo * len, ws, scratch);
+          replay = c.replay_tab;
+        } else {
+          typedef typename T::C C;
+          L(sw_prep_kernel<C>, batch_blocks(m, SW<C>::BATCH), 128, m, d_e + lo * len, d_r + lo * len, d_s + lo * len, ws, scratch);
+          replay = c.sw_replay_tab[curve];
+        }
+        return L.rc;
+      });
+      if (rc2) return rc2;
+      const KeyedVerifyArgs a{d_e + lo * len, d_r + lo * len, d_s + lo * len, d_idx + lo, c.d_status + lo, ws, c.gtab[curve], replay};
+      cudaError_t err = keyset_verify_launch(curve, m, d, a, L.st, c.ev_k0[k], c.ev_k1[k], &L.count);
+      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_verify_launch");
+    },
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {status + lo, c.d_status + lo, m};
+      return 1;
+    });
+}
+}  // namespace
+
+static void keysets_release_all() {
+  std::lock_guard<std::mutex> lk(g_ks_mu);
+  for (eb200_keyset* ks : g_keysets) keyset_free_device(ks);
+  g_keysets.clear();
+}
+
+extern "C" {
+
+int eb200_keyset_create(int curve, size_t m, const uint8_t* pub, uint32_t pub_fmt, uint32_t table_bits,
+                        uint8_t* key_status, eb200_keyset** out) {
+  if (out) *out = nullptr;
+  if (!out || !pub || !key_status || m == 0 || m > 0xffffffffull || !fmt_ok(pub_fmt)) return EB200_ERR_ARG;
+  if (table_bits && (table_bits < EB200_KEYSET_MIN_BITS || table_bits > EB200_KEYSET_MAX_BITS)) return EB200_ERR_ARG;
+  if (!keyset_geom(curve).limbs) return EB200_ERR_UNSUPPORTED;      // the 25519 curves, and unknown ids as elsewhere
+  if (!table_bits && !(table_bits = keyset_choose_bits(curve, m, EB200_KEYSET_DEFAULT_BUDGET))) {
+    snprintf(g_err, sizeof g_err, "the tables of %zu keys do not fit the default budget at any width: pass table_bits", m);
+    return EB200_ERR_ARG;
+  }
+  int devs[MAX_DEV], nd;
+  { std::lock_guard<std::mutex> lk(g_mu); nd = g_ndev; for (int i = 0; i < nd; i++) devs[i] = g_devs[i]; }
+  if (nd == 0) return EB200_ERR_NOT_INIT;
+  eb200_keyset* ks = new eb200_keyset;
+  ks->curve = curve; ks->m = m; ks->W = table_bits; ks->fmt = pub_fmt;
+  ks->device_bytes = 2 * curve_len(curve) * m + m + keyset_key_bytes(curve, (int)table_bits) * m;
+  t_pending = nullptr;
+  eb200_timing tm = {};
+  int rc = EB200_OK;
+  for (int i = 0; i < nd && !rc; i++) {
+    Ctx& c = g_ctx[devs[i]];
+    std::lock_guard<std::mutex> lk(c.mu);
+    cudaError_t e = cudaSetDevice(c.device);
+    if (e != cudaSuccess) { rc = cuda_fail(e, "cudaSetDevice"); break; }
+    ks->devs[ks->ndev++] = c.device;                 // listed first, so that a failed build frees what it allocated
+    c.timing = eb200_timing{};
+    rc = keyset_build_on(c, ks, pub, key_status);
+    merge_timing(tm, c.timing);
+  }
+  t_timing = tm;
+  if (rc) {
+    keyset_free_device(ks);
+    delete ks;
+    return rc;
+  }
+  ks->live = true;
+  { std::lock_guard<std::mutex> lk(g_ks_mu); g_keysets.push_back(ks); }
+  *out = ks;
+  return EB200_OK;
+}
+
+int eb200_keyset_info(const eb200_keyset* ks, int* curve, size_t* m, uint32_t* table_bits, size_t* device_bytes) {
+  if (!ks) return EB200_ERR_ARG;
+  if (curve) *curve = ks->curve;
+  if (m) *m = ks->m;
+  if (table_bits) *table_bits = ks->W;
+  if (device_bytes) *device_bytes = ks->device_bytes;
+  return EB200_OK;
+}
+
+int eb200_keyset_destroy(eb200_keyset* ks) {
+  if (!ks) return EB200_OK;
+  {
+    std::lock_guard<std::mutex> lk(g_ks_mu);
+    for (size_t i = 0; i < g_keysets.size(); i++)
+      if (g_keysets[i] == ks) { g_keysets.erase(g_keysets.begin() + i); break; }
+    if (ks->live) keyset_free_device(ks);
+  }
+  delete ks;
+  return EB200_OK;
+}
+
+int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r,
+                                   const uint8_t* s, const uint32_t* key_idx, uint8_t* status) {
+  if (!ks) return EB200_ERR_ARG;
+  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (n == 0) return EB200_OK;
+  if (!e || !r || !s || !key_idx || !status) return EB200_ERR_ARG;
+  for (size_t i = 0; i < n; i++) if (key_idx[i] >= ks->m) return EB200_ERR_ARG;
+  const size_t len = curve_len(ks->curve);
+  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
+    return verify_keyed_on(c, ks, m, e + lo * len, r + lo * len, s + lo * len, key_idx + lo, status + lo);
   });
 }
 

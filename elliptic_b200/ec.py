@@ -9,6 +9,8 @@ does it; all curve arithmetic happens in libelliptic_b200.so on the GPU.
 """
 import re
 
+import ctypes
+
 import numpy as np
 
 from . import _native as nat
@@ -250,7 +252,15 @@ def parse_der(data):
     return int.from_bytes(r, "big"), int.from_bytes(s, "big")
 
 
-class EC:
+class _KeyObjects:
+    """The key-object side of the `ec` API (ec/key.js), in batch form; EC inherits it."""
+
+    def key_set(self, keys, enc=None, table_bits=0):
+        """The batch form of `key = ec.keyFromPublic(pub, enc)` + `key.getPublic().precompute()`: a KeySet on the GPU."""
+        return KeySet(self, keys, enc, table_bits)
+
+
+class EC(_KeyObjects):
     def __init__(self, curve="secp256k1", device=0):
         if curve not in _CURVES:
             raise EllipticError("Unknown curve " + str(curve))   # ec/index.js:19-20
@@ -646,3 +656,114 @@ class EC:
         if st == nat.ST_NEEDS_HOST:
             raise NeedsReferencePath("public key is not on the curve; the reference does not validate it")
         return _answer(st == nat.ST_TRUE, st, (nat.ST_TRUE, nat.ST_FALSE))
+
+
+class KeySet:
+    """Public keys imported once and kept on the GPU with their precomputed tables (eb200_keyset_create); item i of a
+    verify call is checked against key key_idx[i], with the status EC.verify_batch gives for that key.  Keys come in the
+    reference's argument forms through EC._public; a set that mixes {x, y} / uncompressed keys with compressed ones holds
+    one native set per wire format, so no key is converted (or validated) on the host and every throw stays the engine's.
+    `status`: per key, a throw status, ST_TRUE (on the curve) or ST_FALSE (imported, off the curve).  close() frees the
+    device memory; the object is a context manager."""
+
+    def __init__(self, ec, keys, enc=None, table_bits=0):
+        if ec.name not in _SHORT:
+            raise EllipticError("key_set: short curves only")
+        self._ec = ec
+        lib = nat.init(ec._device)
+        groups = {}                                   # pub format -> (key indices, key bytes)
+        for j, key in enumerate(keys):
+            fmt, pb = ec._public(key, enc)
+            g = groups.setdefault(fmt, ([], []))
+            g[0].append(j)
+            g[1].append(pb)
+        m = len(keys)
+        self.status = np.zeros(m, np.uint8)
+        self._where = np.zeros((m, 2), np.uint32)     # key -> (sub-set, index in it)
+        self._sets = []
+        self.table_bits, self.device_bytes = [], 0
+        try:
+            for fmt, (idx, pbs) in groups.items():
+                pub = np.frombuffer(b"".join(pbs), np.uint8).reshape(len(pbs), -1).copy()
+                st = np.zeros(len(idx), np.uint8)
+                h = ctypes.c_void_p()
+                nat.check(lib.eb200_keyset_create(ec._c["id"], len(idx), pub.ctypes.data, fmt, table_bits, st.ctypes.data,
+                                                  ctypes.byref(h)))
+                self._sets.append(h)
+                self.status[idx] = st
+                self._where[idx, 0] = len(self._sets) - 1
+                self._where[idx, 1] = np.arange(len(idx))
+                w, db = ctypes.c_uint32(), ctypes.c_size_t()
+                nat.check(lib.eb200_keyset_info(h, None, None, ctypes.byref(w), ctypes.byref(db)))
+                self.table_bits.append(w.value)
+                self.device_bytes += db.value
+        except Exception:
+            self.close()
+            raise
+        self.table_bits = self.table_bits[0] if len(set(self.table_bits)) == 1 else tuple(self.table_bits)
+
+    def close(self):
+        lib = nat.load()
+        for h in self._sets:
+            nat.check(lib.eb200_keyset_destroy(h))
+        self._sets = []
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def verify_batch_packed(self, e, r, s, key_idx):
+        """e, r, s: (n, len) uint8 arrays (big-endian); key_idx: n indices into the set.  Returns the status bytes."""
+        lib = nat.load()
+        ln = self._ec._len
+        e, r, s = (np.ascontiguousarray(a, dtype=np.uint8) for a in (e, r, s))
+        key_idx = np.asarray(key_idx)
+        n = e.shape[0]
+        if not (e.shape == (n, ln) and r.shape == e.shape and s.shape == e.shape and key_idx.shape == (n,)):
+            raise ValueError("e, r, s must be (n, %d) uint8 arrays and key_idx (n,)" % ln)
+        if n and (key_idx.min() < 0 or key_idx.max() >= len(self.status)):
+            raise ValueError("key_idx out of range")
+        if not self._sets and n:
+            raise EllipticError("key set is closed")
+        status = np.empty(n, np.uint8)
+        if len(self._sets) == 1:
+            nat.call(lib.eb200_ecdsa_verify_batch_keyed, self._sets[0], n, e, r, s, np.ascontiguousarray(key_idx, np.uint32), status)
+            return status
+        where = self._where[key_idx]
+        for k, h in enumerate(self._sets):
+            sel = np.nonzero(where[:, 0] == k)[0]
+            if len(sel):
+                st = np.empty(len(sel), np.uint8)
+                nat.call(lib.eb200_ecdsa_verify_batch_keyed, h, len(sel), np.ascontiguousarray(e[sel]), np.ascontiguousarray(r[sel]),
+                         np.ascontiguousarray(s[sel]), np.ascontiguousarray(where[sel, 1]), st)
+                status[sel] = st
+        return status
+
+    def verify_batch(self, msgs, sigs, key_idx, enc=None, msg_bit_length=None):
+        """Lists of the reference's message and signature forms, as EC.verify_batch takes them; `enc` is accepted for
+        symmetry (signatures are read as the reference reads them, 'hex')."""
+        ec, n = self._ec, len(msgs)
+        early = {}
+
+        def items():
+            for i in range(n):
+                ev = ec._truncate_to_n(msgs[i], msg_bit_length)
+                rv, sv = _signature(sigs[i], "hex")
+                if rv < 1 or rv >= ec.n or sv < 1 or sv >= ec.n:
+                    early[i] = nat.ST_FALSE
+                    rv = sv = 0
+                yield from (ev, rv, sv)
+        ers = _pack(items(), ec._len).reshape(n, 3, ec._len)
+        st = self.verify_batch_packed(ers[:, 0], ers[:, 1], ers[:, 2], key_idx)
+        for i, v in early.items():
+            if st[i] in (nat.ST_TRUE, nat.ST_FALSE, nat.ST_NEEDS_HOST):
+                st[i] = v
+        return st

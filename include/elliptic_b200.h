@@ -261,6 +261,49 @@ int eb200_curve_validate_batch(const eb200_short_curve* curve, size_t n, const u
 int eb200_eddsa_sign_batch(size_t n, const uint8_t* secrets, const uint8_t* msgs, const uint64_t* msg_off,
                            uint8_t* out_sig, uint8_t* out_pub, uint8_t* status);
 
+/* Key sets: the batch form of the reference's key objects -- `key = ec.keyFromPublic(pub, enc)` once,
+ * `key.getPublic().precompute()` (lib/elliptic/curve/base.js:312-327), then `key.verify(msg, sig)` many times
+ * (lib/elliptic/ec/key.js:20-28, 84-99, 114-116).  A set holds m public keys of one short preset (secp256k1, p256, p384,
+ * p521, p192, p224; the 25519 curves return EB200_ERR_UNSUPPORTED) on the GPU: decoded once, checked against the curve
+ * once, and each on-curve key with a table of its multiples (2i+1) 2^(W j) Q over W-bit windows, so that a keyed verify
+ * needs no doubling and no per-item table.
+ *   pub, pub_fmt : m keys, exactly what eb200_ecdsa_verify_batch takes
+ *   table_bits   : the window width W, EB200_KEYSET_MIN_BITS..EB200_KEYSET_MAX_BITS, or 0 for the widest of them whose
+ *                  tables (m * (floor(mbits / W) + 1) * 2^(W-1) entries of x || y limbs; mbits = 131 on secp256k1, whose
+ *                  windows cover a GLV half, else bits(n) - 1) fit EB200_KEYSET_DEFAULT_BUDGET bytes per device.  If
+ *                  not even the narrowest fits, or for any other value: EB200_ERR_ARG (an explicit width is not held
+ *                  to the budget; there is no silent fallback to the unkeyed path)
+ *   key_status   : m bytes out -- EB200_ST_THROW_* = keyFromPublic throws that error; EB200_ST_TRUE = imported and
+ *                  pub.validate() is true; EB200_ST_FALSE = imported but off the curve ({x, y} and uncompressed keys
+ *                  are not validated by the reference)
+ * The tables are built on every device initialised at the time of the call and the keyed calls stay on those devices;
+ * a device added by a later eb200_init does not serve this set.  A failed allocation returns EB200_ERR_CUDA, leaves
+ * *out NULL and frees what it had allocated.  m = 0, m >= 2^32 or a NULL pointer: EB200_ERR_ARG.
+ * eb200_last_timing after create: kernel_ms = main_kernel_ms = the build kernels of the slowest device; launches = 3
+ * per device (4 with a SEC1 format: the decoder).
+ * A set is read-only once created: several threads may verify against it at once and several sets may be alive.
+ * Destroying a set while a call uses it is the caller's error.  eb200_shutdown frees the device memory of surviving
+ * sets; their handles then answer EB200_ERR_NOT_INIT and must still be passed to eb200_keyset_destroy. */
+#define EB200_KEYSET_MIN_BITS 4
+#define EB200_KEYSET_MAX_BITS 8
+#define EB200_KEYSET_DEFAULT_BUDGET ((size_t)1 << 30)
+typedef struct eb200_keyset eb200_keyset;
+int eb200_keyset_create(int curve, size_t m, const uint8_t* pub, uint32_t pub_fmt, uint32_t table_bits,
+                        uint8_t* key_status, eb200_keyset** out);
+/* Any out pointer may be NULL.  device_bytes: what the set holds on EACH of its devices. */
+int eb200_keyset_info(const eb200_keyset* ks, int* curve, size_t* m, uint32_t* table_bits, size_t* device_bytes);
+int eb200_keyset_destroy(eb200_keyset* ks);          /* NULL is a no-op returning EB200_OK */
+
+/* Batch of key.verify(msg, sig): item i is checked against key key_idx[i] of the set.  e, r, s as
+ * eb200_ecdsa_verify_batch takes them (host pointers, sharded over the set's devices).  status[i] is exactly the byte
+ * eb200_ecdsa_verify_batch writes for the same e, r, s with pub[i] = key key_idx[i] in the set's format: the key's throw
+ * first, then TRUE / FALSE, and for an off-curve key the reference's schedule-dependent answer, replayed on the GPU from
+ * the key's coordinates.  A key_idx[i] >= m returns EB200_ERR_ARG before anything is written.
+ * eb200_last_timing: main_kernel_ms = the keyed main kernel; launches = 3 per chunk (prep, main, replay).
+ * There is no device-pointer (`_dev`) and no DER variant of this call yet. */
+int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r,
+                                   const uint8_t* s, const uint32_t* key_idx, uint8_t* status);
+
 /* Self-test hooks used by the parity tests (device arithmetic vs the oracle).
  * op: 0 mul, 1 sqr, 2 add, 3 sub, 4 neg, 5 mul_small(b[0]), 6 normalize, 7 inv, 8 sqrt candidate.
  * a, b, out: n x 8 little-endian 32-bit limbs (host pointers). */
