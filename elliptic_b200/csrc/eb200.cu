@@ -42,13 +42,13 @@ __global__ void __launch_bounds__(128) k256_gtab_kernel(u32* gtab) {
 __global__ void __launch_bounds__(128) k256_prep_kernel(size_t N, const uint8_t* __restrict__ e,
                                                         const uint8_t* __restrict__ r,
                                                         const uint8_t* __restrict__ s,
-                                                        u32* __restrict__ ws, u32* __restrict__ scratch) {
+                                                        u32* __restrict__ ws, u32* __restrict__ scratch, int batch) {
   size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   size_t T = (size_t)gridDim.x * blockDim.x;
-  prep_thread(tid, T, N, e, r, s, ws, scratch);
+  prep_thread(tid, T, N, e, r, s, ws, scratch, 0, batch);
 }
 
-__global__ void __launch_bounds__(EB_VERIFY_BLOCK, EB_VERIFY_MINBLOCKS)
+__global__ void __launch_bounds__(EB_VERIFY_BLOCK, EB_K256_VERIFY_MINBLOCKS)
 k256_verify_kernel(size_t N, const uint8_t* __restrict__ pub, const uint8_t* __restrict__ r,
                    const u32* __restrict__ ws, const u32* __restrict__ gtab,
                    u32* __restrict__ qtab, const uint8_t* __restrict__ pre, uint8_t* __restrict__ status) {
@@ -645,6 +645,10 @@ struct Launch {
 unsigned blocks128(size_t threads) { return (unsigned)((threads + 127) / 128); }
 // grid of a prep / finish kernel whose threads each take up to `batch` items
 unsigned batch_blocks(size_t n, int batch) { return blocks128((n + batch - 1) / batch); }
+// Items per thread of the secp256k1 verify prep.  Each thread pays one inversion (~300 products mod n) for its
+// batch, so a larger batch amortises it, as long as the grid still fills the GPU: 2^20 items at 32 per thread are
+// 256 blocks of 128.  Smaller calls (and the pipelined host calls' 2^18-item chunks) keep PREP_BATCH.
+int k256_prep_batch(size_t n) { return n >= ((size_t)1 << 20) ? 32 : PREP_BATCH; }
 
 // Which kernels serve a curve id: secp256k1 and ed25519 have their own, the other short curves share the SW<C>
 // templates and sign with their curves.js hash (p384: SHA-384, p521: SHA-512, the rest: SHA-256).
@@ -865,7 +869,7 @@ int launch_verify(Ctx& c, int curve, size_t n, const uint8_t* d_e, const uint8_t
       L(ed_ec_verify_kernel, nb, 128, n, d_e, d_r, d_s, xy, pre, gt, qtab, d_status);
       CK(cudaEventRecord(ev_main1, L.st));
     } else if constexpr (is_k256<T>) {
-      L(k256_prep_kernel, batch_blocks(n, PREP_BATCH), 128, n, d_e, d_r, d_s, ws, scratch);
+      L(k256_prep_kernel, batch_blocks(n, k256_prep_batch(n)), 128, n, d_e, d_r, d_s, ws, scratch, k256_prep_batch(n));
       CK(cudaEventRecord(ev_main0, L.st));
       L(k256_verify_kernel, (unsigned)((n + EB_VERIFY_BLOCK - 1) / EB_VERIFY_BLOCK), EB_VERIFY_BLOCK, n, xy, d_r, ws, gt,
         qtab, pre, d_status);
@@ -2103,7 +2107,8 @@ int verify_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, 
         typedef decltype(cv) T;
         if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;
         else if constexpr (is_k256<T>) {
-          L(k256_prep_kernel, batch_blocks(m, PREP_BATCH), 128, m, d_e + lo * len, d_r + lo * len, d_s + lo * len, ws, scratch);
+          L(k256_prep_kernel, batch_blocks(m, k256_prep_batch(m)), 128, m, d_e + lo * len, d_r + lo * len, d_s + lo * len, ws,
+            scratch, k256_prep_batch(m));
           replay = c.replay_tab;
         } else {
           typedef typename T::C C;

@@ -10,7 +10,7 @@
 //   curve/short.js:908-925            JPoint.eqXToP
 //
 // GPU-first algorithm (same outputs, different schedule):
-//   kernel 1 (prep): Montgomery-trick batch inversion of s over 16 items/thread,
+//   kernel 1 (prep): Montgomery-trick batch inversion of s over 16-32 items/thread,
 //     u1 = e/s, u2 = r/s, GLV split of u2 into odd (k1,k2), regular recoding.
 //   kernel 2 (main): one thread per signature.  Per-item table {1,3,..,15}*Q in
 //     "effective affine" form on an isomorphic curve (shared Z), 33 windows of
@@ -148,7 +148,7 @@ EB_HD void prep_store(size_t i, size_t N, u32* u1, const u32* u2, u32 flags, u32
 }
 
 // ---------------------------------------------------------------------------
-// prep: thread `tid` of `T` handles items tid, tid+T, ... (up to PREP_BATCH).
+// prep: thread `tid` of `T` handles items tid, tid+T, ... (up to `batch` <= 64; T * batch >= N).
 // e, r, s: N x 32 bytes big-endian.  ws: PREP_WORDS x N words.
 // scratch: 8 x N words (prefix products).
 // mode 0 (verify, ec/index.js:199-207): invert s; u1 = e/s, u2 = r/s; r, s outside [1, n-1] -> FALSE.
@@ -157,14 +157,14 @@ EB_HD void prep_store(size_t i, size_t N, u32* u1, const u32* u2, u32 flags, u32
 // mode 2 (getKeyRecoveryParam, recovery_param_item): invert s mod n; u1 = e/s, u2 = (r mod n)/s; no range checks;
 //         s = 0 (mod n) -> FL_INVALID (recovery_param_cold_item decides those items).
 EB_HD void prep_thread(size_t tid, size_t T, size_t N, const uint8_t* e, const uint8_t* r,
-                       const uint8_t* s, u32* ws, u32* scratch, int mode = 0) {
+                       const uint8_t* s, u32* ws, u32* scratch, int mode = 0, int batch = PREP_BATCH) {
   u32 R2[8], one[8], nn[8];
   K256N::r2(R2); K256N::r1(one); K256N::n(nn);
   u32 prod[8];
   copy_n<8>(prod, one);
-  u32 invalid_mask = 0;
+  u64 invalid_mask = 0;
   int cnt = 0;
-  for (int j = 0; j < PREP_BATCH; j++) {
+  for (int j = 0; j < batch; j++) {
     size_t i = tid + (size_t)j * T;
     if (i >= N) break;
     cnt = j + 1;
@@ -180,7 +180,7 @@ EB_HD void prep_thread(size_t tid, size_t T, size_t N, const uint8_t* e, const u
       sc_mont_mul(sm, sv, R2);
       if (mode == 2) ok = !is_zero_n<8>(sm);        // s mod n
     }
-    if (!ok) invalid_mask |= 1u << j;
+    if (!ok) invalid_mask |= (u64)1 << j;
     cmov_n<8>(sm, one, !ok);
     // scratch[i] = prefix product BEFORE this item
     for (int w = 0; w < 8; w++) scratch[(size_t)w * N + i] = prod[w];
@@ -336,47 +336,58 @@ EB_HD ge_jac k256_dsm(size_t i, size_t N, const ge_aff& Q, u32 flags, const u32*
   return gq_to_jac(acc);
 }
 #else
+// Per-item table (2k+1)*Q, k = 0..7, for an ON-CURVE Q: tab[24k..24k+23] = (x, y, beta*x) as affine points on
+// the isomorphic curve y^2 = x^3 + 7*Zg^6 (the a = 0 formulas never use b); returns Zg.  Built with co-Z
+// additions (Meloni): all points of one step share a Z, so no addition needs it.
+EB_HD fe qtab_build(const ge_aff& Q, u32* tab) {
+  // co-Z doubling of the affine Q (dbl-2009-l at Z = 1): D = 2Q and P = Q, both on Z = 2*y(Q), i.e. affine on
+  // the curve scaled by 2*y(Q).  y(Q) != 0: the group has odd order.
+  fe B = fe_sqr(Q.x);
+  fe E = fe_sqr(Q.y);
+  fe L = fe_sqr(E);
+  fe S = fe_dbl(fe_sub(fe_sub(fe_sqr(fe_add(Q.x, E)), B), L));   // 4 x y^2 = x * (2y)^2
+  fe M = fe_add(B, fe_dbl(B));
+  fe L8 = fe_dbl(fe_dbl(fe_dbl(L)));                               // 8 y^4 = y * (2y)^3
+  fe Dx = fe_sub(fe_sqr(M), fe_dbl(S));
+  fe Dy = fe_sub(fe_mul(M, fe_sub(S, Dx)), L8);
+  fe Px = S, Py = L8;
+  store_fe(tab + 0, Px); store_fe(tab + 8, Py);
+  for (int k = 1; k < QTAB_ENTRIES; k++) {
+    // ZADDU: P += D with D moved to the new Z; Z_k = Z_{k-1} * h.  (2k-1)Q = +-2Q is impossible in a group of
+    // large prime order, so h != 0.
+    fe h = fe_sub(Px, Dx);
+    fe C = fe_sqr(h);
+    fe W1 = fe_mul(Px, C), W2 = fe_mul(Dx, C);
+    fe A2 = fe_mul(Dy, fe_sub(W1, W2));                            // y_D * h^3
+    fe dy = fe_sub(Py, Dy);
+    Px = fe_sub(fe_sub(fe_sqr(dy), W1), W2);
+    Py = fe_sub(fe_mul(dy, fe_sub(W2, Px)), A2);
+    Dx = W2; Dy = A2;
+    store_fe(tab + 24 * k, Px); store_fe(tab + 24 * k + 8, Py);
+    store_fe(tab + 24 * k + 16, h);                                // Z_k / Z_{k-1}, consumed below
+  }
+  // rescale every entry to Z = Z_7 and append beta*x
+  fe beta = fe_beta();
+  fe zs = fe_one();
+  for (int k = QTAB_ENTRIES - 1; k >= 0; k--) {
+    fe X = load_fe(tab + 24 * k), Y = load_fe(tab + 24 * k + 8);
+    if (k < QTAB_ENTRIES - 1) {
+      fe zs2 = fe_sqr(zs);
+      fe zs3 = fe_mul(zs2, zs);
+      X = fe_mul(X, zs2);
+      Y = fe_mul(Y, zs3);
+      store_fe(tab + 24 * k, X); store_fe(tab + 24 * k + 8, Y);
+    }
+    if (k > 0) zs = fe_mul(zs, load_fe(tab + 24 * k + 16));
+    store_fe(tab + 24 * k + 16, fe_mul(X, beta));
+  }
+  return fe_mul(zs, fe_dbl(Q.y));                                  // Z_7 * 2y(Q)
+}
+
 // u1*G + u2*Q for an ON-CURVE Q, scalars as prepared by prep_thread in ws.  Jacobian result.
 EB_HD ge_jac k256_dsm(size_t i, size_t N, const ge_aff& Q, u32 flags, const u32* ws, const u32* gtab, u32* qtab) {
-  // ---- per-item table: (2k+1)*Q, k = 0..7, as affine points on an isomorphic
-  // curve y^2 = x^3 + 7*Zg^6 (the a = 0 formulas never use b), Zg = zglobal.
   u32* tab = qtab + (size_t)i * QTAB_WORDS;
-  fe zglobal;
-  {
-    ge_jac D = jac_dbl(jac_from_aff(Q));     // 2Q, finite for an on-curve Q
-    fe C2 = fe_sqr(D.z);
-    fe C3 = fe_mul(C2, D.z);
-    ge_aff Dp; Dp.x = D.x; Dp.y = D.y;       // 2Q is affine on the curve scaled by C = D.z
-    ge_jac P;
-    P.x = fe_mul(Q.x, C2);
-    P.y = fe_mul(Q.y, C3);
-    P.z = fe_one();
-    store_fe(tab + 0, P.x); store_fe(tab + 8, P.y);
-    for (int k = 1; k < QTAB_ENTRIES; k++) {
-      madd_out o = jac_madd_h(P, Dp);
-      P = o.r;
-      store_fe(tab + 24 * k, P.x); store_fe(tab + 24 * k + 8, P.y);
-      store_fe(tab + 24 * k + 16, o.h);      // Z_k / Z_{k-1}, consumed below
-    }
-    zglobal = fe_mul(P.z, D.z);
-    // rescale every entry to Z = Z_7 and append beta*x
-    fe beta = fe_beta();
-    fe zs = fe_one();
-    for (int k = QTAB_ENTRIES - 1; k >= 0; k--) {
-      fe X = load_fe(tab + 24 * k), Y = load_fe(tab + 24 * k + 8);
-      fe hk = fe_one();
-      if (k > 0) hk = load_fe(tab + 24 * k + 16);
-      if (k < QTAB_ENTRIES - 1) {
-        fe zs2 = fe_sqr(zs);
-        fe zs3 = fe_mul(zs2, zs);
-        X = fe_mul(X, zs2);
-        Y = fe_mul(Y, zs3);
-        store_fe(tab + 24 * k, X); store_fe(tab + 24 * k + 8, Y);
-      }
-      store_fe(tab + 24 * k + 16, fe_mul(X, beta));
-      zs = fe_mul(zs, hk);
-    }
-  }
+  fe zglobal = qtab_build(Q, tab);
 
   // ---- u2*Q = k1*Q + k2*(lambda*Q): 33 windows of 4 bits, regular signed-odd digits
   ge_jac acc = jac_infinity();

@@ -7,6 +7,9 @@
 #ifndef EB_VERIFY_MINBLOCKS
 #define EB_VERIFY_MINBLOCKS 3
 #endif
+#ifndef EB_K256_VERIFY_MINBLOCKS
+#define EB_K256_VERIFY_MINBLOCKS 4  // the secp256k1 verify kernel alone: 128 registers, four blocks per SM
+#endif
 #ifndef EB_SW_MINBLOCKS_BIG
 #define EB_SW_MINBLOCKS_BIG 2     // 12- and 18-limb curves (p384, p521): 255 registers
 #endif
