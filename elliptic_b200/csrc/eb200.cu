@@ -195,9 +195,47 @@ __global__ void __launch_bounds__(128) k256_decode_pub_kernel(size_t N, const ui
   pre[i] = st;
 }
 
+// Scalar-field ops 16..21 of the self-test hook (eb200_selftest_fe, include/elliptic_b200.h) on the plain words
+// a, b: the raw Montgomery product takes them as given, so a = R - 1 reaches the multiplier.  Returns false
+// for any other op.
+template <class S>
+__device__ bool selftest_sc(int op, const u32* a, const u32* b, u32* out) {
+  typedef typename S::fe fe_t;
+  fe_t A = load_fe_n<S::N>(a), B = load_fe_n<S::N>(b), R;
+  switch (op) {
+    case 16: R = S::mul(A, B); break;
+    case 17: R = S::to_mont(A); break;
+    case 18: R = S::from_mont(A); break;
+    case 19: R = S::add(A, B); break;
+    case 20: R = S::sub(A, B); break;
+    case 21: R = S::inv(A); break;
+    default: return false;
+  }
+  store_fe_n<S::N>(out, R);
+  return true;
+}
+
 __global__ void k256_selftest_fe_kernel(int op, size_t n, const u32* a, const u32* b, u32* out) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  // mod n: the product, Montgomery conversion and inversion as prep_thread calls them
+  if (op == 16 || op == 17 || op == 18) {
+    u32 m[8] = {1, 0, 0, 0, 0, 0, 0, 0};            // from_mont: times a plain 1
+    if (op == 16) copy_n<8>(m, b + 8 * i);
+    if (op == 17) K256N::r2(m);
+    sc_mont_mul(out + 8 * i, a + 8 * i, m);
+    return;
+  }
+  if (op == 21) { sc_mont_inv(out + 8 * i, a + 8 * i); return; }
+  if (op == 24 || op == 25) {                       // glv_split_odd: m1 (24) or m2 (25), then neg1, neg2
+    u32 m1[5], m2[5];
+    bool n1, n2;
+    glv_split_odd(a + 8 * i, m1, &n1, m2, &n2);
+    for (int w = 0; w < 5; w++) out[8 * i + w] = op == 24 ? m1[w] : m2[w];
+    out[8 * i + 5] = n1; out[8 * i + 6] = n2; out[8 * i + 7] = 0;
+    return;
+  }
+  if (selftest_sc<Fp<K256_FN>>(op, a + 8 * i, b + 8 * i, out + 8 * i)) return;
   fe A = load_fe(a + 8 * i), B = load_fe(b + 8 * i), R;
   switch (op) {
     case 0: R = fe_mul(A, B); break;
@@ -416,6 +454,26 @@ __global__ void sw_selftest_fe_kernel(int op, size_t n, const u32* a, const u32*
   }
   store_fe_n<NL>(out + NL * i, F::from_mont(R));
 }
+// The short curves' other self-test ops: the doubling's scaled products (8..11) and the scalar field (16..21).  A
+// kernel of its own, first named by eb200_selftest_fe at the end of this file: instantiating this code inside
+// sw_selftest_fe_kernel, which sw_kernel_order names early, changed the inlining in sw_mul_add_kernel<P384>.
+template <class C>
+__global__ void sw_selftest_ext_kernel(int op, size_t n, const u32* a, const u32* b, u32* out) {
+  typedef typename SW<C>::F F;
+  constexpr int NL = SW<C>::N;
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (selftest_sc<typename C::S>(op, a + NL * i, b + NL * i, out + NL * i)) return;
+  typename F::fe A = F::to_mont(load_fe_n<NL>(a + NL * i)), B = F::to_mont(load_fe_n<NL>(b + NL * i)), R;
+  switch (op) {            // called as SW::dbl_inl calls them
+    case 8: R = F::template mul_k<3>(A, B); break;
+    case 9: R = F::template mul_k<4>(A, B); break;
+    case 10: R = F::template sqr_k<8>(A); break;
+    case 11: R = F::dbl(A); break;
+    default: R = A;
+  }
+  store_fe_n<NL>(out + NL * i, F::from_mont(R));
+}
 
 // ---------------------------------------------------------------------------
 // ed25519 / curve25519 kernels
@@ -435,6 +493,7 @@ ed25519_verify_kernel(size_t N, const uint8_t* __restrict__ R, const uint8_t* __
 __global__ void f25_selftest_kernel(int op, size_t n, const u32* a, const u32* b, u32* out) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  if (selftest_sc<Fp<ED25519_FN>>(op, a + 8 * i, b + 8 * i, out + 8 * i)) return;   // mod l (ed25519_ec.cuh)
   f25 A = f25_load(a + 8 * i), B = f25_load(b + 8 * i), R;
   switch (op) {
     case 0: R = f25_mul(A, B); break;
@@ -1927,7 +1986,10 @@ int eb200_selftest_fe(int curve, int op, size_t n, const uint32_t* a, const uint
   else with_curve(curve, [&](auto cv) {
     typedef decltype(cv) T;
     if constexpr (is_k256<T>) k256_selftest_fe_kernel<<<nb, 128, 0, c.stream>>>(op, n, da, db, dout);
-    else if constexpr (!is_ed25519<T>) sw_selftest_fe_kernel<typename T::C><<<nb, 128, 0, c.stream>>>(op, n, da, db, dout);
+    else if constexpr (!is_ed25519<T>) {
+      if (op >= 8) sw_selftest_ext_kernel<typename T::C><<<nb, 128, 0, c.stream>>>(op, n, da, db, dout);
+      else sw_selftest_fe_kernel<typename T::C><<<nb, 128, 0, c.stream>>>(op, n, da, db, dout);
+    }
     return EB200_OK;
   });
   CK(cudaGetLastError());

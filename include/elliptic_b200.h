@@ -305,8 +305,20 @@ int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8
                                    const uint8_t* s, const uint32_t* key_idx, uint8_t* status);
 
 /* Self-test hooks used by the parity tests (device arithmetic vs the oracle).
- * op: 0 mul, 1 sqr, 2 add, 3 sub, 4 neg, 5 mul_small(b[0]), 6 normalize, 7 inv, 8 sqrt candidate.
- * a, b, out: n x 8 little-endian 32-bit limbs (host pointers). */
+ * a, b, out: n elements of L little-endian 32-bit limbs each (host pointers); L = 8, except p192 6, p384 12 and
+ * p521 18.  An op the curve does not know returns a (short curves) or 0 (secp256k1, ed25519 / curve25519).
+ * Coordinate field, on plain integers:
+ *   0 mul, 1 sqr, 2 add, 3 sub, 4 neg, 7 inv (all curves);
+ *   secp256k1 and the 25519 curves (weakly reduced results): 5 mul_small(b[0]), 6 normalize, 8 sqrt candidate
+ *     (secp256k1) / a^((p-5)/8) (25519);
+ *   p192 .. p521 (canonical results): 8 3ab, 9 4ab, 10 8a^2, 11 2a -- mul_k<3>, mul_k<4>, sqr_k<8> and dbl as the
+ *     doubling calls them.
+ * Scalar field mod n (mod l on the 25519 curves), on the words as given, Montgomery radix R = 2^(32 L):
+ *   16 a b R^-1 (a < R, b < n), 17 to Montgomery form (a R mod n), 18 from Montgomery form (a R^-1 mod n),
+ *   19 add, 20 sub (canonical operands), 21 inverse in Montgomery form (a^(n-2) R^(3-n) mod n; 0 -> 0).
+ *   On secp256k1 ops 16, 17, 18 and 21 run sc_mont_mul / sc_mont_inv, the calls of the verify prep.
+ * secp256k1 GLV split of a (< n) into odd halves k1 + k2 lambda = a (mod n), |ki| = 2 mi + 1:
+ *   24 writes m1, 25 writes m2 (limbs 0..4), then the signs of k1 and k2 (limbs 5, 6: 1 = negative), limb 7 = 0. */
 int eb200_selftest_fe(int curve, int op, size_t n, const uint32_t* a, const uint32_t* b, uint32_t* out);
 /* Geometry of the fixed-base table: entry (j, i) = (2i+1) * 2^(wbits*j) * G, 16 words (x||y limbs). */
 int eb200_selftest_gtab_dims(int curve, int* windows, int* entries, int* wbits);
