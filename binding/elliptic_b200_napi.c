@@ -335,6 +335,18 @@ static void keyset_finalize(napi_env env, void* data, void* hint) {
   eb200_keyset_destroy(b->ks);
   free(b);
 }
+/* the result object of a create call (rc: its return code; the box is freed on failure) */
+static napi_value keyset_out(napi_env env, int rc, keyset_box* b, napi_value status) {
+  if (rc) { free(b); return fail(env, rc); }
+  uint32_t w = 0; size_t bytes = 0;
+  eb200_keyset_info(b->ks, 0, 0, &w, &bytes);
+  napi_value o = obj(env), h, vw, vb;
+  napi_create_external(env, b, keyset_finalize, 0, &h);
+  napi_create_uint32(env, w, &vw);
+  napi_create_double(env, (double)bytes, &vb);
+  SET(o, "handle", h); SET(o, "status", status); SET(o, "tableBits", vw); SET(o, "deviceBytes", vb);
+  return o;
+}
 static napi_value KeysetCreate(napi_env env, napi_callback_info info) {
   ARGS(4); I32(0, curve); BUF(1, pub, lp); U32(2, fmt); U32(3, bits);
   size_t len = field_len(curve), pb = pub_bytes(len, fmt);
@@ -345,15 +357,18 @@ static napi_value KeysetCreate(napi_env env, napi_callback_info info) {
   if (!b) return fail(env, EB200_ERR_ARG);
   uint8_t* st; napi_value arr = out_u8(env, m, &st);
   int rc = eb200_keyset_create(curve, m, pub, fmt, bits, st, &b->ks);
-  if (rc) { free(b); return fail(env, rc); }
-  uint32_t w = 0; size_t bytes = 0;
-  eb200_keyset_info(b->ks, 0, 0, &w, &bytes);
-  napi_value o = obj(env), h, vw, vb;
-  napi_create_external(env, b, keyset_finalize, 0, &h);
-  napi_create_uint32(env, w, &vw);
-  napi_create_double(env, (double)bytes, &vb);
-  SET(o, "handle", h); SET(o, "status", arr); SET(o, "tableBits", vw); SET(o, "deviceBytes", vb);
-  return o;
+  return keyset_out(env, rc, b, arr);
+}
+/* eddsaKeysetCreate(A: m x 32 encoded keys, tableBits) -> {handle, status: Uint8Array(m), tableBits, deviceBytes} */
+static napi_value EddsaKeysetCreate(napi_env env, napi_callback_info info) {
+  ARGS(2); BUF(0, A, la); U32(1, bits);
+  size_t m = la / 32;
+  if (la % 32) return fail(env, EB200_ERR_ARG);
+  keyset_box* b = (keyset_box*)calloc(1, sizeof *b);
+  if (!b) return fail(env, EB200_ERR_ARG);
+  uint8_t* st; napi_value arr = out_u8(env, m, &st);
+  int rc = eb200_eddsa_keyset_create(m, A, bits, st, &b->ks);
+  return keyset_out(env, rc, b, arr);
 }
 /* keysetDestroy(handle): frees the set now; the handle stays valid and answers EB200_ERR_ARG afterwards */
 static napi_value KeysetDestroy(napi_env env, napi_callback_info info) {
@@ -382,6 +397,28 @@ static napi_value EcdsaVerifyBatchKeyed(napi_env env, napi_callback_info info) {
   return rc ? fail(env, rc) : arr;
 }
 
+/* eddsaVerifyBatchKeyed(handle, R, S, h | null, msgs | null, msgOff | null, keyIdx: Uint8Array over n little-endian
+ * uint32) -> Uint8Array(n) of statuses   (eddsa.verify against keys of an EdDSA set; h as eddsaVerifyBatch) */
+static napi_value EddsaVerifyBatchKeyed(napi_env env, napi_callback_info info) {
+  ARGS(7); BUF(1, R, a); BUF(2, S, b); OPT(3, h, d); OPT(4, msgs, lm); OPT(5, off, lo); BUF(6, idx, li);
+  void* p = 0;
+  if (napi_get_value_external(env, argv[0], &p) != napi_ok || !p || !((keyset_box*)p)->ks) return fail(env, EB200_ERR_ARG);
+  eb200_keyset* ks = ((keyset_box*)p)->ks;
+  size_t n = a / 32;
+  if (a % 32 || b != a || li != 4 * n || ((uintptr_t)idx & 3) || (h && d != a) ||
+      (!h && (lo != 8 * (n + 1) || ((uintptr_t)off & 7)))) return fail(env, EB200_ERR_ARG);
+  if (!h) {
+    const uint64_t* o = (const uint64_t*)off;
+    for (size_t i = 0; i < n; i++) if (o[i + 1] < o[i]) return fail(env, EB200_ERR_ARG);
+    if (o[n] > lm) return fail(env, EB200_ERR_ARG);
+  }
+  const uint32_t* ki = (const uint32_t*)(const void*)idx;
+  uint8_t* st; napi_value arr = out_u8(env, n, &st);
+  int rc = h ? eb200_eddsa_verify_batch_keyed(ks, n, R, S, h, ki, st)
+             : eb200_eddsa_verify_batch_keyed_msgs(ks, n, R, S, msgs, (const uint64_t*)off, ki, st);
+  return rc ? fail(env, rc) : arr;
+}
+
 static napi_value Register(napi_env env, napi_value exports) {
   static const struct { const char* name; napi_callback cb; } fns[] = {
       {"init", Init}, {"ecdsaVerifyBatch", EcdsaVerifyBatch}, {"ecdsaVerifyBatchAsync", EcdsaVerifyBatchAsync},
@@ -390,7 +427,8 @@ static napi_value Register(napi_env env, napi_value exports) {
       {"mulAddBatch", MulAddBatch}, {"ecdhDeriveBatch", EcdhDeriveBatch},
       {"curveOpBatch", CurveOpBatch}, {"eddsaVerifyBatch", EddsaVerifyBatch}, {"eddsaSignBatch", EddsaSignBatch},
       {"x25519Batch", X25519Batch},
-      {"keysetCreate", KeysetCreate}, {"keysetDestroy", KeysetDestroy}, {"ecdsaVerifyBatchKeyed", EcdsaVerifyBatchKeyed}};
+      {"keysetCreate", KeysetCreate}, {"keysetDestroy", KeysetDestroy}, {"ecdsaVerifyBatchKeyed", EcdsaVerifyBatchKeyed},
+      {"eddsaKeysetCreate", EddsaKeysetCreate}, {"eddsaVerifyBatchKeyed", EddsaVerifyBatchKeyed}};
   for (unsigned i = 0; i < sizeof fns / sizeof fns[0]; i++) {
     napi_value f;
     napi_create_function(env, fns[i].name, NAPI_AUTO_LENGTH, fns[i].cb, 0, &f);

@@ -4,7 +4,7 @@
 // run on the GPU through the N-API addon -> libelliptic_b200.so (include/elliptic_b200.h):
 //   EC#verifyBatch / verifyBatchAsync / signBatch / genKeyPairBatch / recoverPubKeyBatch / getKeyRecoveryParamBatch /
 //   deriveBatch
-//   EDDSA#verifyBatch / signBatch
+//   EDDSA#verifyBatch / signBatch / keySet
 //   curve.short#mulBatch / mulAddBatch / addBatch / dblBatch / validateBatch   (any parameters, presets take the tuned kernels)
 //   curve.edwards#mulBatch / mulAddBatch (ed25519), curve.mont#mulBatch (curve25519)
 // All parsing (hex / byte arrays / DER / SEC1, _truncateToN) is done by the reference's own JS, so accept / reject /
@@ -279,6 +279,32 @@ elliptic.eddsa.prototype.verifyBatch = function verifyBatch(messages, sigs, pubs
   }
   var m = concatMsgs(ms);
   return Array.prototype.map.call(native.eddsaVerifyBatch(R, S, A, null, m.blob, m.off), statusToBool);
+};
+// EDDSA#keySet(pubs) -> {status, tableBits, deviceBytes, verifyBatch(messages, sigs, keyIdx), destroy()}: the batch form
+// of `key = eddsa.keyFromPublic(pub)` once and eddsa.verify(msg, sig, key) many times.  The keys' bytes (pubBytes(), as
+// given for a key made from bytes) are kept on the GPU with their tables; SHA-512 of R || A || M runs there too.
+elliptic.eddsa.prototype.keySet = function keySet(pubs) {
+  init();
+  var self = this;
+  var keys = pubs.map(function(k) { return self.keyFromPublic(k); });
+  var set = native.eddsaKeysetCreate(pack(keys, 32, function(k) { return k.pubBytes(); }), 0);
+  return {
+    status: set.status, tableBits: set.tableBits, deviceBytes: set.deviceBytes,
+    verifyBatch: function(messages, sigs, keyIdx) {
+      var n = messages.length, R = new Uint8Array(32 * n), S = new Uint8Array(32 * n), idx = new Uint32Array(n), ms = [];
+      for (var i = 0; i < n; i++) {
+        if (!(keyIdx[i] >= 0 && keyIdx[i] < keys.length)) throw new Error('key index out of range');
+        idx[i] = keyIdx[i];
+        var sig = self.makeSignature(sigs[i]);                         // asserts the size (eddsa/signature.js:23-24)
+        R.set(sig.Rencoded(), 32 * i); S.set(sig.Sencoded(), 32 * i);
+        ms.push(elliptic.utils.parseBytes(messages[i]));
+      }
+      var m = concatMsgs(ms);
+      return Array.prototype.map.call(native.eddsaVerifyBatchKeyed(set.handle, R, S, null, m.blob, m.off, new Uint8Array(idx.buffer)),
+        statusToBool);
+    },
+    destroy: function() { native.keysetDestroy(set.handle); }
+  };
 };
 // EDDSA#signBatch(messages, secrets) -> Array<Signature>   (eddsa/index.js:34-44; 32-byte secrets)
 elliptic.eddsa.prototype.signBatch = function signBatch(messages, secrets) {

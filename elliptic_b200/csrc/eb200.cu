@@ -2189,6 +2189,117 @@ int verify_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, 
       return 1;
     });
 }
+
+// ---- EdDSA (ed25519) key sets: kernels in eddsa_keyset.cu, the hash kernel of this file --------------------------------
+// One device's copy: raw keys up, classify + tables, verdicts home.
+int ed_keyset_build_on(Ctx& c, eb200_keyset* ks, const uint8_t* A, uint8_t* key_status) {
+  const size_t m = ks->m;
+  const int W = (int)ks->W;
+  int rc;
+  KeysetDev& d = ks->dev[c.device];
+  d.W = W;
+  CK(cudaMalloc(&d.xy, 32 * m));
+  CK(cudaMalloc(&d.kst, m));
+  CK(cudaMalloc(&d.tab, ed_keyset_key_bytes(W) * m));
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, m * ed_keyset_windows(W) * 24 * 4))) return rc;
+  return run_single(c, {{d.xy, A, 32 * m}},
+    [&](Launch& L) {
+      cudaError_t err = ed_keyset_build_launch(m, d, (u32*)c.d_ws, L.st, &L.count);
+      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "ed_keyset_build_launch");
+    },
+    {{key_status, d.kst, m}}, {}, true);
+}
+
+// Keyed EdDSA verify of one block on one device of the set, chunked like eddsa_on.  h == NULL: raw messages (msg_off
+// points at this block's first offset, offsets absolute); the keys' raw bytes are gathered and hashed on the GPU.
+int eddsa_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* R, const uint8_t* S, const uint8_t* h,
+                   const uint8_t* msgs, const uint64_t* msg_off, const u32* key_idx, uint8_t* status) {
+  const KeysetDev& d = ks->dev[c.device];
+  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
+  int rc = ensure_table(c, EB200_CURVE_ED25519);
+  if (rc) return rc;
+  const ChunkPlan P = make_plan(n);
+  size_t mbytes = h ? 0 : (size_t)(msg_off[n] - msg_off[0]);
+  size_t off_bytes = h ? 0 : (n + 1) * sizeof(uint64_t);
+  size_t base = align256(n * 132);                 // R | S | h | gathered keys | key_idx
+  if ((rc = grow(&c.d_in, &c.d_in_cap, base + align256(off_bytes) + align256(mbytes + 1)))) return rc;
+  if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
+  uint8_t *dR = c.d_in, *dS = dR + 32 * n, *dh = dS + 32 * n, *dA = dh + 32 * n;
+  u32* didx = (u32*)(dA + 32 * n);
+  uint64_t* doff = (uint64_t*)(c.d_in + base);
+  uint8_t* dm = c.d_in + base + align256(off_bytes);
+  const u32* gt = c.gtab[EB200_CURVE_ED25519];
+  return run_chunked(c, P,
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {dR + 32 * lo, R + 32 * lo, 32 * m};
+      seg[1] = {dS + 32 * lo, S + 32 * lo, 32 * m};
+      seg[2] = {didx + lo, key_idx + lo, 4 * m};
+      if (h) { seg[3] = {dh + 32 * lo, h + 32 * lo, 32 * m}; return 4; }
+      seg[3] = {doff + lo, msg_off + lo, (m + 1) * sizeof(uint64_t)};
+      seg[4] = {dm + (msg_off[lo] - msg_off[0]), msgs + msg_off[lo], (size_t)(msg_off[lo + m] - msg_off[lo])};
+      return 5;
+    },
+    [&](size_t lo, size_t m, Launch& L, int, int k) {
+      cudaError_t err;
+      if (!h) {
+        if ((err = ed_keyset_gather_launch(m, d, didx + lo, dA + 32 * lo, L.st, &L.count)) != cudaSuccess)
+          return cuda_fail(err, "ed_keyset_gather_launch");
+        L(ed25519_hash_kernel, blocks128(m), 128, m, dR + 32 * lo, dA + 32 * lo, dm - msg_off[0], doff + lo, dh + 32 * lo);
+        if (L.rc) return L.rc;
+      }
+      CK(cudaEventRecord(c.ev_k0[k], L.st));
+      if ((err = ed_keyset_verify_launch(m, d, dR + 32 * lo, dS + 32 * lo, dh + 32 * lo, didx + lo, gt, c.d_status + lo, L.st,
+                                         &L.count)) != cudaSuccess)
+        return cuda_fail(err, "ed_keyset_verify_launch");
+      CK(cudaEventRecord(c.ev_k1[k], L.st));
+      return EB200_OK;
+    },
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {status + lo, c.d_status + lo, m};
+      return 1;
+    });
+}
+
+// h < n for a 32-byte little-endian h (the keyed tables cover 253 bits)
+bool ed_scalar_below_n(const uint8_t* h) {
+  static const uint8_t n_le[32] = {0xed, 0xd3, 0xf5, 0x5c, 0x1a, 0x63, 0x12, 0x58, 0xd6, 0x9c, 0xf7, 0xa2, 0xde, 0xf9, 0xde, 0x14,
+                                   0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0x10};
+  for (int b = 31; b >= 0; b--)
+    if (h[b] != n_le[b]) return h[b] < n_le[b];
+  return false;
+}
+
+// Builds the set on every initialised device (build(ctx) per device) and registers it; on failure frees what was
+// allocated and deletes ks.  eb200_last_timing: the slowest device's build, launches summed.
+template <class Build>
+int keyset_create_on_devices(eb200_keyset* ks, eb200_keyset** out, Build&& build) {
+  int devs[MAX_DEV], nd;
+  { std::lock_guard<std::mutex> lk(g_mu); nd = g_ndev; for (int i = 0; i < nd; i++) devs[i] = g_devs[i]; }
+  if (nd == 0) { delete ks; return EB200_ERR_NOT_INIT; }
+  t_pending = nullptr;
+  eb200_timing tm = {};
+  int rc = EB200_OK;
+  for (int i = 0; i < nd && !rc; i++) {
+    Ctx& c = g_ctx[devs[i]];
+    std::lock_guard<std::mutex> lk(c.mu);
+    cudaError_t e = cudaSetDevice(c.device);
+    if (e != cudaSuccess) { rc = cuda_fail(e, "cudaSetDevice"); break; }
+    ks->devs[ks->ndev++] = c.device;                 // listed first, so that a failed build frees what it allocated
+    c.timing = eb200_timing{};
+    rc = build(c);
+    merge_timing(tm, c.timing);
+  }
+  t_timing = tm;
+  if (rc) {
+    keyset_free_device(ks);
+    delete ks;
+    return rc;
+  }
+  ks->live = true;
+  { std::lock_guard<std::mutex> lk(g_ks_mu); g_keysets.push_back(ks); }
+  *out = ks;
+  return EB200_OK;
+}
 }  // namespace
 
 static void keysets_release_all() {
@@ -2209,35 +2320,10 @@ int eb200_keyset_create(int curve, size_t m, const uint8_t* pub, uint32_t pub_fm
     snprintf(g_err, sizeof g_err, "the tables of %zu keys do not fit the default budget at any width: pass table_bits", m);
     return EB200_ERR_ARG;
   }
-  int devs[MAX_DEV], nd;
-  { std::lock_guard<std::mutex> lk(g_mu); nd = g_ndev; for (int i = 0; i < nd; i++) devs[i] = g_devs[i]; }
-  if (nd == 0) return EB200_ERR_NOT_INIT;
   eb200_keyset* ks = new eb200_keyset;
   ks->curve = curve; ks->m = m; ks->W = table_bits; ks->fmt = pub_fmt;
   ks->device_bytes = 2 * curve_len(curve) * m + m + keyset_key_bytes(curve, (int)table_bits) * m;
-  t_pending = nullptr;
-  eb200_timing tm = {};
-  int rc = EB200_OK;
-  for (int i = 0; i < nd && !rc; i++) {
-    Ctx& c = g_ctx[devs[i]];
-    std::lock_guard<std::mutex> lk(c.mu);
-    cudaError_t e = cudaSetDevice(c.device);
-    if (e != cudaSuccess) { rc = cuda_fail(e, "cudaSetDevice"); break; }
-    ks->devs[ks->ndev++] = c.device;                 // listed first, so that a failed build frees what it allocated
-    c.timing = eb200_timing{};
-    rc = keyset_build_on(c, ks, pub, key_status);
-    merge_timing(tm, c.timing);
-  }
-  t_timing = tm;
-  if (rc) {
-    keyset_free_device(ks);
-    delete ks;
-    return rc;
-  }
-  ks->live = true;
-  { std::lock_guard<std::mutex> lk(g_ks_mu); g_keysets.push_back(ks); }
-  *out = ks;
-  return EB200_OK;
+  return keyset_create_on_devices(ks, out, [&](Ctx& c) { return keyset_build_on(c, ks, pub, key_status); });
 }
 
 int eb200_keyset_info(const eb200_keyset* ks, int* curve, size_t* m, uint32_t* table_bits, size_t* device_bytes) {
@@ -2263,7 +2349,7 @@ int eb200_keyset_destroy(eb200_keyset* ks) {
 
 int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r,
                                    const uint8_t* s, const uint32_t* key_idx, uint8_t* status) {
-  if (!ks) return EB200_ERR_ARG;
+  if (!ks || ks->curve == EB200_CURVE_ED25519) return EB200_ERR_ARG;      // an EdDSA set: eb200_eddsa_verify_batch_keyed
   if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
   if (n == 0) return EB200_OK;
   if (!e || !r || !s || !key_idx || !status) return EB200_ERR_ARG;
@@ -2271,6 +2357,47 @@ int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8
   const size_t len = curve_len(ks->curve);
   return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
     return verify_keyed_on(c, ks, m, e + lo * len, r + lo * len, s + lo * len, key_idx + lo, status + lo);
+  });
+}
+
+int eb200_eddsa_keyset_create(size_t m, const uint8_t* A, uint32_t table_bits, uint8_t* key_status, eb200_keyset** out) {
+  if (out) *out = nullptr;
+  if (!out || !A || !key_status || m == 0 || m > 0xffffffffull) return EB200_ERR_ARG;
+  if (table_bits && (table_bits < EB200_KEYSET_MIN_BITS || table_bits > EB200_KEYSET_MAX_BITS)) return EB200_ERR_ARG;
+  if (!table_bits && !(table_bits = ed_keyset_choose_bits(m, EB200_KEYSET_DEFAULT_BUDGET))) {
+    snprintf(g_err, sizeof g_err, "the tables of %zu keys do not fit the default budget at any width: pass table_bits", m);
+    return EB200_ERR_ARG;
+  }
+  eb200_keyset* ks = new eb200_keyset;
+  ks->curve = EB200_CURVE_ED25519; ks->m = m; ks->W = table_bits;
+  ks->device_bytes = 32 * m + m + ed_keyset_key_bytes((int)table_bits) * m;
+  return keyset_create_on_devices(ks, out, [&](Ctx& c) { return ed_keyset_build_on(c, ks, A, key_status); });
+}
+
+int eb200_eddsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* R, const uint8_t* S, const uint8_t* h,
+                                   const uint32_t* key_idx, uint8_t* status) {
+  if (!ks || ks->curve != EB200_CURVE_ED25519) return EB200_ERR_ARG;
+  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (n == 0) return EB200_OK;
+  if (!R || !S || !h || !key_idx || !status) return EB200_ERR_ARG;
+  for (size_t i = 0; i < n; i++) if (key_idx[i] >= ks->m || !ed_scalar_below_n(h + 32 * i)) return EB200_ERR_ARG;
+  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
+    return eddsa_keyed_on(c, ks, m, R + 32 * lo, S + 32 * lo, h + 32 * lo, nullptr, nullptr, key_idx + lo, status + lo);
+  });
+}
+
+int eb200_eddsa_verify_batch_keyed_msgs(const eb200_keyset* ks, size_t n, const uint8_t* R, const uint8_t* S,
+                                        const uint8_t* msgs, const uint64_t* msg_off, const uint32_t* key_idx,
+                                        uint8_t* status) {
+  if (!ks || ks->curve != EB200_CURVE_ED25519) return EB200_ERR_ARG;
+  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (n == 0) return EB200_OK;
+  if (!R || !S || !msg_off || !key_idx || !status || (!msgs && msg_off[n])) return EB200_ERR_ARG;
+  for (size_t i = 0; i < n; i++) if (msg_off[i + 1] < msg_off[i] || key_idx[i] >= ks->m) return EB200_ERR_ARG;
+  static const uint8_t none = 0;
+  const uint8_t* mp = msgs ? msgs : &none;
+  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
+    return eddsa_keyed_on(c, ks, m, R + 32 * lo, S + 32 * lo, nullptr, mp, msg_off + lo, key_idx + lo, status + lo);
   });
 }
 

@@ -7,7 +7,8 @@
 
 // One device's copy of a key set: m keys decoded to x || y (2 len bytes each), keyFromPublic's verdict per key
 // (a throw status, EB200_ST_TRUE = on the curve, EB200_ST_FALSE = imported but off the curve) and the tables of the
-// on-curve keys, keyset_key_bytes() apart, W bits per window.
+// on-curve keys, keyset_key_bytes() apart, W bits per window.  An ed25519 set (eddsa_keyset.cu) keeps the 32 raw bytes
+// of each key in `xy`, its verdict (EB200_ST_TRUE or the decoder's throw) in `kst` and ed_keyset_key_bytes() per key.
 struct KeysetDev {
   uint8_t* xy;
   uint8_t* kst;
@@ -33,3 +34,14 @@ struct KeyedVerifyArgs {
 // adds the kernels launched (two) to *launches.  Other curve ids launch nothing and return cudaErrorInvalidValue.
 cudaError_t keyset_verify_launch(int curve, size_t n, const KeysetDev& k, const KeyedVerifyArgs& a, cudaStream_t st,
                                  cudaEvent_t main_begin, cudaEvent_t main_end, unsigned* launches);
+
+// ed25519 (eddsa_keyset.cu).  Build: classifies the m raw keys in k.xy and builds their tables on `st`; bases: scratch of
+// m * ed_keyset_windows(W) * 24 words.  Adds the kernels launched (three) to *launches.
+cudaError_t ed_keyset_build_launch(size_t m, const KeysetDev& k, uint32_t* bases, cudaStream_t st, unsigned* launches);
+// Writes the raw bytes of key key_idx[i] to A_out[32 i ..] for the hash kernel (one kernel).
+cudaError_t ed_keyset_gather_launch(size_t n, const KeysetDev& k, const uint32_t* key_idx, uint8_t* A_out, cudaStream_t st,
+                                    unsigned* launches);
+// The keyed main kernel: R, S, h (n x 32, h < n) and key_idx in, status out; gtab: the ed25519 fixed-base table.
+cudaError_t ed_keyset_verify_launch(size_t n, const KeysetDev& k, const uint8_t* R, const uint8_t* S, const uint8_t* h,
+                                    const uint32_t* key_idx, const uint32_t* gtab, uint8_t* status, cudaStream_t st,
+                                    unsigned* launches);

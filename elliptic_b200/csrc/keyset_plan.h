@@ -37,3 +37,17 @@ static inline uint32_t keyset_choose_bits(int curve, size_t m, size_t budget) {
   }
   return 0;
 }
+
+// ed25519 key sets (eb200_eddsa_keyset_create) have a geometry of their own: entry (j, i) = i 2^(W j) (-A) for
+// i = 1 .. 2^(W-1), affine niels (y+x, y-x, 2d x y), 24 words.  The windows cover every h < n < 2^253 with signed
+// digits in [-2^(W-1), 2^(W-1)) and an unsigned top digit, which stays <= 2^(W-1) for W = 4..8.
+constexpr int ED_KS_ENTRY_WORDS = 24;
+static inline int ed_keyset_windows(int W) { return (253 + W - 1) / W; }
+static inline size_t ed_keyset_key_bytes(int W) {
+  return (size_t)ed_keyset_windows(W) * ((size_t)1 << (W - 1)) * ED_KS_ENTRY_WORDS * 4;
+}
+static inline uint32_t ed_keyset_choose_bits(size_t m, size_t budget) {
+  for (int W = EB200_KEYSET_MAX_BITS; W >= EB200_KEYSET_MIN_BITS; W--)
+    if (m <= budget / ed_keyset_key_bytes(W)) return (uint32_t)W;
+  return 0;
+}

@@ -658,7 +658,32 @@ class EC(_KeyObjects):
         return _answer(st == nat.ST_TRUE, st, (nat.ST_TRUE, nat.ST_FALSE))
 
 
-class KeySet:
+class _NativeSets:
+    """The lifecycle of key-set handles (eb200_keyset) shared by KeySet and eddsa.EdKeySet: `_sets` holds the live
+    handles; close() destroys them (the object is then closed), the object is a context manager and closes on
+    collection."""
+    _sets = ()
+
+    def close(self):
+        lib = nat.load()
+        for h in self._sets:
+            nat.check(lib.eb200_keyset_destroy(h))
+        self._sets = []
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class KeySet(_NativeSets):
     """Public keys imported once and kept on the GPU with their precomputed tables (eb200_keyset_create); item i of a
     verify call is checked against key key_idx[i], with the status EC.verify_batch gives for that key.  Keys come in the
     reference's argument forms through EC._public; a set that mixes {x, y} / uncompressed keys with compressed ones holds
@@ -701,24 +726,6 @@ class KeySet:
             self.close()
             raise
         self.table_bits = self.table_bits[0] if len(set(self.table_bits)) == 1 else tuple(self.table_bits)
-
-    def close(self):
-        lib = nat.load()
-        for h in self._sets:
-            nat.check(lib.eb200_keyset_destroy(h))
-        self._sets = []
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def verify_batch_packed(self, e, r, s, key_idx):
         """e, r, s: (n, len) uint8 arrays (big-endian); key_idx: n indices into the set.  Returns the status bytes."""

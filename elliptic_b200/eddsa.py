@@ -6,12 +6,13 @@ argument forms and error behaviour (eddsa/index.js:52-63) and `verify_batch` is 
 batch entry point.  Byte/hex parsing and the SHA-512 of R || A || M are done here
 (hashlib; the reference uses hash.js); all curve arithmetic runs on the GPU.
 """
+import ctypes
 import hashlib
 
 import numpy as np
 
 from . import _native as nat
-from .ec import EllipticError, _answer, _blob, _pack, _to_array
+from .ec import EllipticError, _NativeSets, _answer, _blob, _pack, _to_array
 
 N_ED25519 = 0x1000000000000000000000000000000014DEF9DEA2F79CD65812631A5CF5D3ED
 
@@ -21,7 +22,15 @@ def _parse_bytes(x):
     return _to_array(x, "hex") if isinstance(x, str) else _to_array(x)
 
 
-class EDDSA:
+class _EdKeyObjects:
+    """The key-object side of the `eddsa` API (eddsa/key.js), in batch form; EDDSA inherits it."""
+
+    def key_set(self, pubs, table_bits=0):
+        """The batch form of `key = eddsa.keyFromPublic(pub)` for many keys: an EdKeySet on the GPU."""
+        return EdKeySet(self, pubs, table_bits)
+
+
+class EDDSA(_EdKeyObjects):
     def __init__(self, curve="ed25519", device=0):
         if curve != "ed25519":
             raise EllipticError("only tested with ed25519 so far")      # eddsa/index.js:12
@@ -63,6 +72,19 @@ class EDDSA:
         nat.call(lib.eb200_eddsa_verify_batch_msgs, n, R, S, A, msgs if msgs.size else None, msg_off, status)
         return status
 
+    def _signature(self, sig):
+        sig = _parse_bytes(sig)
+        if len(sig) != 2 * self.encoding_length:
+            raise EllipticError("Signature has invalid size")       # eddsa/signature.js:23-24
+        return sig
+
+    def _pub(self, pub):
+        pub = _parse_bytes(pub)
+        if len(pub) != self.encoding_length:
+            # decodePoint on another length reads a different y; not on the accelerated path
+            raise EllipticError("unsupported public key length %d" % len(pub))
+        return pub
+
     def verify_batch(self, messages, sigs, pubs, gpu_hash=True):
         """EDDSA#verifyBatch: lists of the reference's own argument forms (hex strings / byte arrays).
         gpu_hash=False computes hashInt with hashlib on the host instead of on the GPU."""
@@ -71,13 +93,8 @@ class EDDSA:
         for i in range(n):
             if not gpu_hash:
                 ms.append(_parse_bytes(messages[i]))      # the host path reads the message first
-            sig = _parse_bytes(sigs[i])
-            if len(sig) != 2 * self.encoding_length:
-                raise EllipticError("Signature has invalid size")       # eddsa/signature.js:23-24
-            pub = _parse_bytes(pubs[i])
-            if len(pub) != self.encoding_length:
-                # decodePoint on another length reads a different y; not on the accelerated path
-                raise EllipticError("unsupported public key length %d" % len(pub))
+            sig = self._signature(sigs[i])
+            pub = self._pub(pubs[i])
             rsa.append(sig + pub)
             if gpu_hash:
                 ms.append(_parse_bytes(messages[i]))
@@ -134,3 +151,85 @@ class EDDSA:
         """EDDSA.prototype.verify (eddsa/index.js:52-63): bool, or raises."""
         st = int(self.verify_batch([message], [sig], [pub])[0])
         return _answer(st == nat.ST_TRUE, st, (nat.ST_TRUE, nat.ST_FALSE))
+
+
+class EdKeySet(_NativeSets):
+    """ed25519 public keys imported once and kept on the GPU, raw bytes and per-key tables (eb200_eddsa_keyset_create);
+    item i of a verify call is checked against key key_idx[i], with the status EDDSA.verify_batch gives for that key.
+    `status`: per key, ST_TRUE (the key decodes) or the throw of decoding it.  close() frees the device memory; the
+    object is a context manager."""
+
+    def __init__(self, ed, pubs, table_bits=0):
+        self._ed = ed
+        A = np.frombuffer(b"".join(ed._pub(p) for p in pubs), np.uint8).reshape(len(pubs), 32).copy()
+        self._A = A
+        lib = nat.init(ed._device)
+        m = len(pubs)
+        self.status = np.zeros(m, np.uint8)
+        h = ctypes.c_void_p()
+        nat.check(lib.eb200_eddsa_keyset_create(m, A.ctypes.data, table_bits, self.status.ctypes.data, ctypes.byref(h)))
+        self._sets = [h]
+        w, db = ctypes.c_uint32(), ctypes.c_size_t()
+        nat.check(lib.eb200_keyset_info(h, None, None, ctypes.byref(w), ctypes.byref(db)))
+        self.table_bits, self.device_bytes = w.value, db.value
+
+    def _args(self, R, S, key_idx):
+        R, S = (np.ascontiguousarray(a, dtype=np.uint8) for a in (R, S))
+        key_idx = np.asarray(key_idx)
+        n = R.shape[0]
+        if not (R.shape == (n, 32) and S.shape == R.shape and key_idx.shape == (n,)):
+            raise ValueError("R, S must be (n, 32) uint8 arrays and key_idx (n,)")
+        if n and (key_idx.min() < 0 or key_idx.max() >= len(self.status)):
+            raise ValueError("key_idx out of range")
+        return R, S, np.ascontiguousarray(key_idx, np.uint32), n
+
+    def _handle(self):
+        if not self._sets:
+            raise EllipticError("key set is closed")
+        return self._sets[0]
+
+    def verify_batch_packed(self, R, S, h, key_idx):
+        """R, S, h: (n, 32) uint8 arrays (little-endian wire forms; h = hashInt(R, A, M) < n); key_idx: n indices into
+        the set.  Returns the status bytes."""
+        R, S, key_idx, n = self._args(R, S, key_idx)
+        h = np.ascontiguousarray(h, dtype=np.uint8)
+        if h.shape != (n, 32):
+            raise ValueError("h must be an (n, 32) uint8 array")
+        status = np.empty(n, np.uint8)
+        if n:
+            nat.call(nat.load().eb200_eddsa_verify_batch_keyed, self._handle(), n, R, S, h, key_idx, status)
+        return status
+
+    def verify_batch_msgs_packed(self, R, S, msgs, msg_off, key_idx):
+        """Like verify_batch_packed but takes the raw messages (concatenated bytes + n+1 offsets); the key bytes are
+        gathered, hashed with R and the message, and reduced mod n on the GPU."""
+        R, S, key_idx, n = self._args(R, S, key_idx)
+        msgs = np.ascontiguousarray(msgs, dtype=np.uint8)
+        msg_off = np.ascontiguousarray(msg_off, dtype=np.uint64)
+        if not (msg_off.shape == (n + 1,) and int(msg_off[n]) == msgs.size):
+            raise ValueError("msg_off must hold n + 1 offsets, the last one equal to len(msgs)")
+        status = np.empty(n, np.uint8)
+        if n:
+            nat.call(nat.load().eb200_eddsa_verify_batch_keyed_msgs, self._handle(), n, R, S, msgs if msgs.size else None,
+                     msg_off, key_idx, status)
+        return status
+
+    def verify_batch(self, messages, sigs, key_idx, gpu_hash=True):
+        """Lists of the reference's message and signature forms, as EDDSA.verify_batch takes them, against keys of the
+        set.  gpu_hash=False computes hashInt with hashlib on the host (over the key's raw bytes) instead."""
+        ed, n = self._ed, len(messages)
+        if len(sigs) != n or len(key_idx) != n:
+            raise ValueError("messages, sigs and key_idx must have the same length")
+        ms, sig = [], []
+        for i in range(n):                                # each item read in EDDSA.verify_batch's order
+            if not gpu_hash:
+                ms.append(_parse_bytes(messages[i]))
+            sig.append(ed._signature(sigs[i]))
+            if gpu_hash:
+                ms.append(_parse_bytes(messages[i]))
+        rs = np.frombuffer(b"".join(sig), np.uint8).reshape(n, 64)
+        if gpu_hash:
+            return self.verify_batch_msgs_packed(rs[:, :32], rs[:, 32:], *_blob(ms), key_idx)
+        R, S, idx, _ = self._args(rs[:, :32], rs[:, 32:], key_idx)
+        h = _pack([ed.hash_int(sig[i][:32], self._A[idx[i]], ms[i]) for i in range(n)], 32, "little")
+        return self.verify_batch_packed(R, S, h, idx)

@@ -264,7 +264,8 @@ int eb200_eddsa_sign_batch(size_t n, const uint8_t* secrets, const uint8_t* msgs
 /* Key sets: the batch form of the reference's key objects -- `key = ec.keyFromPublic(pub, enc)` once,
  * `key.getPublic().precompute()` (lib/elliptic/curve/base.js:312-327), then `key.verify(msg, sig)` many times
  * (lib/elliptic/ec/key.js:20-28, 84-99, 114-116).  A set holds m public keys of one short preset (secp256k1, p256, p384,
- * p521, p192, p224; the 25519 curves return EB200_ERR_UNSUPPORTED) on the GPU: decoded once, checked against the curve
+ * p521, p192, p224; the 25519 curves return EB200_ERR_UNSUPPORTED here, and ed25519 EdDSA keys have
+ * eb200_eddsa_keyset_create below) on the GPU: decoded once, checked against the curve
  * once, and each on-curve key with a table of its multiples (2i+1) 2^(W j) Q over W-bit windows, so that a keyed verify
  * needs no doubling and no per-item table.
  *   pub, pub_fmt : m keys, exactly what eb200_ecdsa_verify_batch takes
@@ -303,6 +304,35 @@ int eb200_keyset_destroy(eb200_keyset* ks);          /* NULL is a no-op returnin
  * There is no device-pointer (`_dev`) and no DER variant of this call yet. */
 int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r,
                                    const uint8_t* s, const uint32_t* key_idx, uint8_t* status);
+
+/* EdDSA key sets: `key = eddsa.keyFromPublic(bytes)` once, then `eddsa.verify(msg, sig, key)` many times
+ * (lib/elliptic/eddsa/index.js:52-63, eddsa/key.js:17-44), on ed25519.  The handle is the same eb200_keyset: _info
+ * reports EB200_CURVE_ED25519, _destroy and eb200_shutdown treat it as any other set, and passing it to
+ * eb200_ecdsa_verify_batch_keyed (or an ECDSA set to the calls below) returns EB200_ERR_ARG.
+ *   A          : m x 32 encoded public keys, kept as given (hashInt reads key.pubBytes(), which for a key made from
+ *                bytes is those bytes, a non-canonical y >= p included)
+ *   table_bits : W = EB200_KEYSET_MIN_BITS..EB200_KEYSET_MAX_BITS, or 0 for the widest whose tables fit
+ *                EB200_KEYSET_DEFAULT_BUDGET bytes per device; a key's table is ceil(253 / W) windows of 2^(W-1) affine
+ *                niels entries i 2^(W j) (-A) of 96 bytes (W = 7: 227,328 bytes, 4,723 keys per GiB).  Otherwise as
+ *                eb200_keyset_create: no width fits -> EB200_ERR_ARG, an explicit width is not held to the budget.
+ *   key_status : m bytes out -- EB200_ST_TRUE = the key decodes, else the throw of decoding it (THROW_INVALID_POINT,
+ *                THROW_ASSERT).  There is no FALSE verdict: a decoded key is on the curve.
+ * m = 0, m >= 2^32 or a NULL pointer: EB200_ERR_ARG; no device: EB200_ERR_NOT_INIT; a failed allocation: EB200_ERR_CUDA
+ * with *out NULL and everything freed.  device_bytes = 32 m + m + the tables.  eb200_last_timing after create: the
+ * build kernels of the slowest device; launches = 3 per device (classify, window bases, table windows). */
+int eb200_eddsa_keyset_create(size_t m, const uint8_t* A, uint32_t table_bits, uint8_t* key_status, eb200_keyset** out);
+/* Batch of eddsa.verify against the set: item i uses key key_idx[i].  R, S, h as eb200_eddsa_verify_batch takes them;
+ * status[i] is the byte eb200_eddsa_verify_batch writes for the same R, S, h and A = that key's bytes, in the reference's
+ * order: S >= n -> FALSE, then R's throw, then the key's, then TRUE / FALSE.  A key_idx[i] >= m or an h[i] >= n returns
+ * EB200_ERR_ARG before anything is written.  Host pointers, sharded over the set's devices and chunked as the unkeyed
+ * call.  eb200_last_timing: main_kernel_ms = the keyed main kernel; launches = 1 per chunk. */
+int eb200_eddsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* R, const uint8_t* S, const uint8_t* h,
+                                   const uint32_t* key_idx, uint8_t* status);
+/* Same from raw messages, as eb200_eddsa_verify_batch_msgs takes them: h = SHA512(R || A_raw[key_idx[i]] || M) mod n on
+ * the GPU.  launches = 3 per chunk (key-byte gather, hash, keyed main). */
+int eb200_eddsa_verify_batch_keyed_msgs(const eb200_keyset* ks, size_t n, const uint8_t* R, const uint8_t* S,
+                                        const uint8_t* msgs, const uint64_t* msg_off, const uint32_t* key_idx,
+                                        uint8_t* status);
 
 /* Self-test hooks used by the parity tests (device arithmetic vs the oracle).
  * a, b, out: n elements of L little-endian 32-bit limbs each (host pointers); L = 8, except p192 6, p384 12 and
