@@ -397,6 +397,51 @@ static napi_value EcdsaVerifyBatchKeyed(napi_env env, napi_callback_info info) {
   return rc ? fail(env, rc) : arr;
 }
 
+/* the ECDSA set behind a handle and its field length, or 0 */
+static eb200_keyset* ecdsa_set(napi_env env, napi_value v, size_t* len) {
+  void* p = 0;
+  int curve = 0;
+  if (napi_get_value_external(env, v, &p) != napi_ok || !p || !((keyset_box*)p)->ks) return 0;
+  eb200_keyset_info(((keyset_box*)p)->ks, &curve, 0, 0, 0);
+  *len = curve == EB200_CURVE_ED25519 ? 0 : field_len(curve);
+  return *len ? ((keyset_box*)p)->ks : 0;
+}
+/* mulAddBatchKeyed(handle, k1 | null, k2, keyIdx: Uint8Array over n little-endian uint32) -> {points, status}
+ * k1 null: pub.mul(k2) (short.js:422-432); else G.mulAdd(k1, pub, k2) (short.js:434-441), pub = key keyIdx[i] */
+static napi_value MulAddBatchKeyed(napi_env env, napi_callback_info info) {
+  ARGS(4); OPT(1, k1, l1); BUF(2, k2, l2); BUF(3, idx, li);
+  size_t len = 0;
+  eb200_keyset* ks = ecdsa_set(env, argv[0], &len);
+  if (!ks) return fail(env, EB200_ERR_ARG);
+  size_t n = li / 4;
+  if (li != 4 * n || l2 != n * len || (k1 && l1 != l2) || ((uintptr_t)idx & 3)) return fail(env, EB200_ERR_ARG);
+  const uint32_t* ki = (const uint32_t*)(const void*)idx;
+  uint8_t *out, *st;
+  napi_value ao = out_u8(env, 2 * len * n, &out), ast = out_u8(env, n, &st);
+  int rc = k1 ? eb200_mul_add_batch_keyed(ks, n, k1, k2, ki, out, st) : eb200_scalar_mul_batch_keyed(ks, n, k2, ki, out, st);
+  if (rc) return fail(env, rc);
+  napi_value res = obj(env);
+  SET(res, "points", ao); SET(res, "status", ast);
+  return res;
+}
+/* ecdhDeriveBatchKeyed(handle, priv, keyIdx: Uint8Array over n little-endian uint32) -> {out, status}
+ * (KeyPair.derive, ec/key.js:102-107, against key keyIdx[i]) */
+static napi_value EcdhDeriveBatchKeyed(napi_env env, napi_callback_info info) {
+  ARGS(3); BUF(1, k, lk); BUF(2, idx, li);
+  size_t len = 0;
+  eb200_keyset* ks = ecdsa_set(env, argv[0], &len);
+  if (!ks) return fail(env, EB200_ERR_ARG);
+  size_t n = li / 4;
+  if (li != 4 * n || lk != n * len || ((uintptr_t)idx & 3)) return fail(env, EB200_ERR_ARG);
+  uint8_t *out, *st;
+  napi_value ao = out_u8(env, lk, &out), ast = out_u8(env, n, &st);
+  int rc = eb200_ecdh_derive_batch_keyed(ks, n, k, (const uint32_t*)(const void*)idx, out, st);
+  if (rc) return fail(env, rc);
+  napi_value res = obj(env);
+  SET(res, "out", ao); SET(res, "status", ast);
+  return res;
+}
+
 /* eddsaVerifyBatchKeyed(handle, R, S, h | null, msgs | null, msgOff | null, keyIdx: Uint8Array over n little-endian
  * uint32) -> Uint8Array(n) of statuses   (eddsa.verify against keys of an EdDSA set; h as eddsaVerifyBatch) */
 static napi_value EddsaVerifyBatchKeyed(napi_env env, napi_callback_info info) {
@@ -428,7 +473,8 @@ static napi_value Register(napi_env env, napi_value exports) {
       {"curveOpBatch", CurveOpBatch}, {"eddsaVerifyBatch", EddsaVerifyBatch}, {"eddsaSignBatch", EddsaSignBatch},
       {"x25519Batch", X25519Batch},
       {"keysetCreate", KeysetCreate}, {"keysetDestroy", KeysetDestroy}, {"ecdsaVerifyBatchKeyed", EcdsaVerifyBatchKeyed},
-      {"eddsaKeysetCreate", EddsaKeysetCreate}, {"eddsaVerifyBatchKeyed", EddsaVerifyBatchKeyed}};
+      {"eddsaKeysetCreate", EddsaKeysetCreate}, {"eddsaVerifyBatchKeyed", EddsaVerifyBatchKeyed},
+      {"mulAddBatchKeyed", MulAddBatchKeyed}, {"ecdhDeriveBatchKeyed", EcdhDeriveBatchKeyed}};
   for (unsigned i = 0; i < sizeof fns / sizeof fns[0]; i++) {
     napi_value f;
     napi_create_function(env, fns[i].name, NAPI_AUTO_LENGTH, fns[i].cb, 0, &f);

@@ -97,9 +97,13 @@ elliptic.ec.prototype.verifyBatchWire = function verifyBatchWire(hashes, ders, k
   return Array.prototype.map.call(st, function(v, i) { return v === 4 ? self.verify(hashes[i], ders[i], keys[i]) : statusToBool(v); });
 };
 
-// EC#keySet(pubs[, enc]) -> {status, tableBits, deviceBytes, verifyBatch(msgs, sigs, keyIdx[, options]), destroy()}: the
-// batch form of `key = ec.keyFromPublic(pub, enc); key.getPublic().precompute()` once and key.verify(msg, sig) many times.
-// The keys are imported here (a key that throws, throws here, as keyFromPublic does) and kept on the GPU with their tables.
+// EC#keySet(pubs[, enc]) -> {status, tableBits, deviceBytes, verifyBatch(msgs, sigs, keyIdx[, options]), mul(keyIdx, ks),
+// mulAdd(k1s, keyIdx, k2s), derive(privs, keyIdx), destroy()}: the batch form of `key = ec.keyFromPublic(pub, enc);
+// key.getPublic().precompute()` once and key.verify(msg, sig), pub.mul(k), G.mulAdd(k1, pub, k2) (Arrays of Points) and
+// keyPair.derive(pub) (an Array of BN) many times.  The keys are imported here (a key that throws, throws here, as
+// keyFromPublic does) and kept on the GPU with their tables.  mul and mulAdd take their scalars as Short#mulBatch and
+// Short#mulAddBatch do, and an off-curve key's result is theirs for that point, not the reference's precomputed-point
+// schedule.
 elliptic.ec.prototype.keySet = function keySet(pubs, enc) {
   var id = curveId(this), self = this, len = this.curve.p.byteLength();
   if (id === undefined || this.curve.type !== 'short') throw new Error('key sets: short preset curves only');
@@ -124,8 +128,34 @@ elliptic.ec.prototype.keySet = function keySet(pubs, enc) {
       var st = native.ecdsaVerifyBatchKeyed(set.handle, e, r, s, new Uint8Array(idx.buffer));
       return Array.prototype.map.call(st, function(v, i) { return i in early ? false : statusToBool(v); });
     },
+    mul: function(keyIdx, ks) {
+      var big = new BN(1).ushln(8 * len);          // Short#mulBatch's rule: only a k of 2^(8 len) or more is reduced mod n
+      var k = pack(ks, len, function(v) { v = new BN(v, 16); return be(v.cmp(big) >= 0 ? v.umod(self.n) : v, len); });
+      return pointsOut(self.curve, native.mulAddBatchKeyed(set.handle, null, k, keyIndices(keyIdx)), ks.length, len);
+    },
+    mulAdd: function(k1s, keyIdx, k2s) {
+      return pointsOut(self.curve, native.mulAddBatchKeyed(set.handle, pack(k1s, len, scalar), pack(k2s, len, scalar), keyIndices(keyIdx)),
+        k1s.length, len);
+    },
+    derive: function(privs, keyIdx) {
+      var res = native.ecdhDeriveBatchKeyed(set.handle, pack(privs, len, scalar), keyIndices(keyIdx)), out = [];
+      for (var i = 0; i < privs.length; i++) {
+        if (res.status[i] !== 1) throw new Error(THROW[res.status[i]]);
+        out.push(new BN(res.out.subarray(len * i, len * i + len)));
+      }
+      return out;
+    },
     destroy: function() { native.keysetDestroy(set.handle); }
   };
+  function scalar(v) { return be(new BN(v, 16).umod(self.n), len); }
+  function keyIndices(keyIdx) {
+    var idx = new Uint32Array(keyIdx.length);
+    for (var i = 0; i < keyIdx.length; i++) {
+      if (!(keyIdx[i] >= 0 && keyIdx[i] < keys.length)) throw new Error('key index out of range');
+      idx[i] = keyIdx[i];
+    }
+    return new Uint8Array(idx.buffer);
+  }
 };
 
 // EC#signBatch(msgs, keys[, enc][, options]) -> Array<Signature>.  options: canonical, pers / persEnc (one string for the

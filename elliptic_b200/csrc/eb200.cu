@@ -2190,6 +2190,73 @@ int verify_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, 
     });
 }
 
+// Keyed Point.mul / G.mulAdd / KeyPair.derive of one block on one device of the set, chunked like verify_keyed_on.
+// k1 == NULL: k2 times the key (derive: x only, and an off-curve key is THROW_NOT_VALIDATED instead of replayed);
+// else k1 G + k2 times the key.  Launches per chunk: prep_scalars, keyed main, normalisation, then the keyed replay
+// (derive: the status map).  derive: the private scalars, their digit words and the Jacobian results are cleared on
+// the chunk's stream behind its kernels, as x25519_on does.
+int mul_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* k1, const uint8_t* k2, const u32* key_idx,
+                 uint8_t* out, uint8_t* status, bool derive) {
+  const int curve = ks->curve;
+  const KeysetDev& d = ks->dev[c.device];
+  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
+  int rc = ensure_table(c, curve);
+  if (rc) return rc;
+  const size_t len = curve_len(curve), ol = derive ? len : 2 * len, limbs = (size_t)keyset_geom(curve).limbs;
+  const ChunkPlan P = make_plan(n);
+  const size_t idx_bytes = align256(n * 4), k_bytes = align256(n * len);
+  if ((rc = grow(&c.d_in, &c.d_in_cap, idx_bytes + 2 * k_bytes + n * ol + 256))) return rc;
+  const WsLayout W = ws_layout(curve, P.max_m);
+  const size_t ws_slot = align256(W.qtab + 3 * limbs * P.max_m * 4);   // prep words | inversion scratch | Jacobian results
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, (P.chunks > 1 ? 2 : 1) * ws_slot))) return rc;
+  if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
+  u32* d_idx = (u32*)c.d_in;
+  uint8_t *d_k1 = c.d_in + idx_bytes, *d_k2 = d_k1 + k_bytes, *d_out = d_k2 + k_bytes;
+  return run_chunked(c, P,
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {d_k2 + lo * len, k2 + lo * len, m * len};
+      seg[1] = {d_idx + lo, key_idx + lo, m * 4};
+      seg[2] = {d_k1 + lo * len, k1 ? k1 + lo * len : nullptr, k1 ? m * len : 0};
+      return 3;
+    },
+    [&](size_t lo, size_t m, Launch& L, int slot, int k) {
+      uint8_t* base = c.d_ws + (size_t)slot * ws_slot;
+      u32 *ws = (u32*)(base + W.ws), *scratch = (u32*)(base + W.scratch), *jac = (u32*)(base + W.qtab);
+      const uint8_t* dk1 = k1 ? d_k1 + lo * len : nullptr;
+      const u32* replay = nullptr;
+      int batch = 0;
+      int rc2 = with_curve(curve, [&](auto cv) {
+        typedef decltype(cv) T;
+        if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;
+        else if constexpr (is_k256<T>) {
+          L(k256_prep_scalars_kernel, blocks128(m), 128, m, dk1, d_k2 + lo * len, ws);
+          replay = c.replay_tab;
+          batch = k256_prep_batch(m);
+        } else {
+          L(sw_prep_scalars_kernel<typename T::C>, blocks128(m), 128, m, dk1, d_k2 + lo * len, ws);
+          replay = c.sw_replay_tab[curve];
+        }
+        return L.rc;
+      });
+      if (rc2) return rc2;
+      const KeyedMulArgs a{dk1, d_k2 + lo * len, d_idx + lo, ws, jac, scratch, c.gtab[curve], replay, d_out + lo * ol,
+                           c.d_status + lo, batch, derive};
+      cudaError_t err = keyset_mul_launch(curve, m, d, a, L.st, c.ev_k0[k], c.ev_k1[k], &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "keyset_mul_launch");
+      if (derive) {
+        L(status_map_kernel, blocks128(m), 128, m, c.d_status + lo, (uint8_t)ST_NEEDS_HOST, (uint8_t)ST_THROW_NOT_VALIDATED);
+        CK(cudaMemsetAsync(d_k2 + lo * len, 0, m * len, L.st));     // the private scalars
+        CK(cudaMemsetAsync(base, 0, ws_slot, L.st));                 // their digit words and the Jacobian results
+      }
+      return L.rc;
+    },
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {out + lo * ol, d_out + lo * ol, m * ol};
+      seg[1] = {status + lo, c.d_status + lo, m};
+      return 2;
+    });
+}
+
 // ---- EdDSA (ed25519) key sets: kernels in eddsa_keyset.cu, the hash kernel of this file --------------------------------
 // One device's copy: raw keys up, classify + tables, verdicts home.
 int ed_keyset_build_on(Ctx& c, eb200_keyset* ks, const uint8_t* A, uint8_t* key_status) {
@@ -2358,6 +2425,39 @@ int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8
   return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
     return verify_keyed_on(c, ks, m, e + lo * len, r + lo * len, s + lo * len, key_idx + lo, status + lo);
   });
+}
+
+}  // extern "C"
+
+// The three keyed multiplication calls: their argument checks, then the set's devices.
+static int mul_keyed_common(const eb200_keyset* ks, size_t n, const uint8_t* k1, const uint8_t* k2, const uint32_t* key_idx,
+                            uint8_t* out, uint8_t* status, bool need_k1, bool derive) {
+  if (!ks || ks->curve == EB200_CURVE_ED25519) return EB200_ERR_ARG;
+  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (n == 0) return EB200_OK;
+  if (!k2 || (need_k1 && !k1) || !key_idx || !out || !status) return EB200_ERR_ARG;
+  for (size_t i = 0; i < n; i++) if (key_idx[i] >= ks->m) return EB200_ERR_ARG;
+  const size_t len = curve_len(ks->curve), ol = derive ? len : 2 * len;
+  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
+    return mul_keyed_on(c, ks, m, k1 ? k1 + lo * len : nullptr, k2 + lo * len, key_idx + lo, out + lo * ol, status + lo, derive);
+  });
+}
+
+extern "C" {
+
+int eb200_scalar_mul_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* k, const uint32_t* key_idx, uint8_t* out_xy,
+                                 uint8_t* status) {
+  return mul_keyed_common(ks, n, nullptr, k, key_idx, out_xy, status, false, false);
+}
+
+int eb200_mul_add_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* k1, const uint8_t* k2, const uint32_t* key_idx,
+                              uint8_t* out_xy, uint8_t* status) {
+  return mul_keyed_common(ks, n, k1, k2, key_idx, out_xy, status, true, false);
+}
+
+int eb200_ecdh_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* priv, const uint32_t* key_idx, uint8_t* out_x,
+                                  uint8_t* status) {
+  return mul_keyed_common(ks, n, nullptr, priv, key_idx, out_x, status, false, true);
 }
 
 int eb200_eddsa_keyset_create(size_t m, const uint8_t* A, uint32_t table_bits, uint8_t* key_status, eb200_keyset** out) {

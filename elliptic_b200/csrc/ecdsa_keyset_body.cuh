@@ -104,6 +104,45 @@ EB_HD void k256_ks_window_item(size_t t, const uint8_t* kst, int W, int windows,
   }
 }
 
+// u2*Q = k1*Q + k2*(lambda*Q) from one key's table `tab`: one mixed add per window and half, regular signed-odd digits.
+// The keyed mul body's accumulation; k256_verify_keyed_item keeps its own copy of these loops, because calling these
+// force-inlined helpers from it changes the code generated for the keyed verify kernels.
+EB_HD ge_jac k256_ks_key_part(size_t i, size_t N, u32 flags, int W, int windows, const u32* tab, const u32* ws) {
+  const fe beta = fe_beta();
+  ge_jac acc = jac_infinity();
+  for (int w = windows - 1; w >= 0; w--) {
+    for (int h = 0; h < 2; h++) {
+      bool dneg;
+      u32 idx = ks_digit(ks_chunk(ws, N, i, h ? 13 : 8, 5, W * w, W), w == windows - 1, W, &dneg);
+      const bool neg = ((flags & (h ? FL_NEG2 : FL_NEG1)) != 0) != dneg;
+      u32 ent[16];
+      ks_load_entry<16>(ent, tab + (((size_t)w << (W - 1)) + idx) * 16);
+      ge_aff P;
+      P.x = load_fe(ent);
+      P.y = load_fe(ent + 8);
+      if (h) P.x = fe_mul(P.x, beta);
+      P = aff_neg_if(P, neg);
+      if (w == windows - 1 && h == 0) acc = jac_from_aff(P);   // the accumulator starts from the first entry
+      else acc = jac_madd(acc, P);
+    }
+  }
+  return acc;
+}
+// acc + u1*G from the fixed table, as k256_dsm
+EB_HD ge_jac k256_ks_g_part(ge_jac acc, size_t i, size_t N, u32 flags, const u32* ws, const u32* gtab) {
+  for (int j = 0; j < GTAB_WINDOWS; j++) {
+    bool dneg;
+    u32 idx = ks_digit(ks_chunk(ws, N, i, 0, 8, GTAB_W * j, GTAB_W), j == GTAB_WINDOWS - 1, GTAB_W, &dneg);
+    bool neg = dneg != ((flags & FL_NEGG) != 0);
+    const u32* ent = gtab + ((size_t)j * GTAB_ENTRIES + idx) * 16;
+    ge_aff P;
+    P.x = load_fe(ent);
+    P.y = load_fe(ent + 8);
+    acc = jac_madd(acc, aff_neg_if(P, neg));
+  }
+  return acc;
+}
+
 // key.verify for item i against key key_idx[i] of the set.  The status eb200_ecdsa_verify_batch gives with that key:
 // the key's throw first, FALSE for r, s out of range, ST_NEEDS_HOST for an off-curve key (the keyed replay kernel
 // then runs the reference's own schedule on the key's coordinates).
@@ -161,6 +200,79 @@ EB_HD uint8_t k256_verify_keyed_item(size_t i, size_t N, const u32* key_idx, con
     if (fe_eq(acc.x, fe_mul(rn, z2))) return ST_TRUE;
   }
   return ST_FALSE;
+}
+
+// Point.mul / G.mulAdd for item i on key key_idx[i] (k2 Q, plus k1 G unless FL_NOG), scalars as
+// k256_prep_scalars_kernel stores them.  The Jacobian result goes to jout word-major (coordinate c, word w at
+// jout[(8 c + w) N + i]), Z = 0 for an item that has no result here.  Status: the key's throw, ST_NEEDS_HOST for an
+// off-curve key (the keyed replay then runs the unkeyed call's schedule), else ST_TRUE; k256_ks_norm_thread turns
+// ST_TRUE into the affine point or ST_INFINITY.
+EB_HD uint8_t k256_mul_keyed_item(size_t i, size_t N, const u32* key_idx, const uint8_t* kst, int W, int windows,
+                                  const u32* ktab, const u32* ws, const u32* gtab, u32* jout) {
+  const u32 k = key_idx[i];
+  const uint8_t ks = kst[k];
+  ge_jac acc = jac_infinity();
+  if (ks == ST_TRUE) {
+    u32 flags = ws[(size_t)18 * N + i];
+    acc = k256_ks_key_part(i, N, flags, W, windows, ktab + ((size_t)k * windows << (W - 1)) * 16, ws);
+    if (!(flags & FL_NOG)) acc = k256_ks_g_part(acc, i, N, flags, ws, gtab);
+  }
+  for (int w = 0; w < 8; w++) {
+    jout[(size_t)w * N + i] = acc.x.v[w];
+    jout[(size_t)(8 + w) * N + i] = acc.y.v[w];
+    jout[(size_t)(16 + w) * N + i] = acc.z.v[w];
+  }
+  return ks == ST_TRUE ? ST_TRUE : ks == ST_FALSE ? ST_NEEDS_HOST : ks;
+}
+
+// Jacobian -> affine big-endian for items tid, tid + T, ... (up to `batch` <= 64, T * batch >= N) with one inversion
+// (Montgomery's trick): the items whose status is ST_TRUE and whose Z != 0 form the product chain; the others are
+// skipped, their output zeroed, and a ST_TRUE item with Z = 0 becomes ST_INFINITY.  xonly: 32 bytes x per item (derive),
+// else x || y.  scratch: 8 x N words (prefix products).
+EB_HD void k256_ks_norm_thread(size_t tid, size_t T, size_t N, int batch, const u32* jac, u32* scratch, bool xonly,
+                               uint8_t* out, uint8_t* status) {
+  const size_t ob = xonly ? 32 : 64;
+  fe prod = fe_one();
+  u64 live = 0;
+  int cnt = 0;
+  for (int j = 0; j < batch; j++) {
+    size_t i = tid + (size_t)j * T;
+    if (i >= N) break;
+    cnt = j + 1;
+    fe z;
+    for (int w = 0; w < 8; w++) z.v[w] = jac[(size_t)(16 + w) * N + i];
+    if (status[i] != ST_TRUE || fe_is_zero(z)) continue;
+    live |= (u64)1 << j;
+    for (int w = 0; w < 8; w++) scratch[(size_t)w * N + i] = prod.v[w];
+    prod = fe_mul(prod, z);
+  }
+  if (cnt == 0) return;
+  fe inv = fe_inv(prod);
+  for (int j = cnt - 1; j >= 0; j--) {
+    size_t i = tid + (size_t)j * T;
+    uint8_t* o = out + ob * i;
+    if (!((live >> j) & 1)) {
+      for (size_t b = 0; b < ob; b++) o[b] = 0;
+      if (status[i] == ST_TRUE) status[i] = ST_INFINITY;
+      continue;
+    }
+    fe x, y, z, pre;
+    for (int w = 0; w < 8; w++) {
+      x.v[w] = jac[(size_t)w * N + i];
+      y.v[w] = jac[(size_t)(8 + w) * N + i];
+      z.v[w] = jac[(size_t)(16 + w) * N + i];
+      pre.v[w] = scratch[(size_t)w * N + i];
+    }
+    fe zi = fe_mul(inv, pre);          // Z_i^-1
+    inv = fe_mul(inv, z);              // drop Z_i from the running inverse
+    fe zi2 = fe_sqr(zi);
+    fe ax = fe_normalize(fe_mul(x, zi2));
+    store_be<8>(o, ax.v);
+    if (!xonly) {
+      fe ay = fe_normalize(fe_mul(fe_mul(y, zi2), zi));
+      store_be<8>(o + 32, ay.v);
+    }
+  }
 }
 
 // The same three steps on the a = -3 presets, in SW<C>'s Montgomery form (entries canonical, like its G table).
@@ -237,6 +349,41 @@ struct SWKeyed {
     }
   }
 
+  // u2*Q from one key's table `tab`: one mixed add per window.  The keyed mul body's accumulation (verify_keyed_item
+  // keeps its own copy, as k256_verify_keyed_item does)
+  static EB_HD jac key_part(size_t i, size_t cnt_items, u32 flags, int W, int windows, const u32* tab, const u32* ws) {
+    jac acc = W_::infinity();
+    for (int w = windows - 1; w >= 0; w--) {
+      bool dneg;
+      u32 idx = ks_digit(ks_chunk(ws, cnt_items, i, N, N, W * w, W), w == windows - 1, W, &dneg);
+      const bool neg = ((flags & W_::FL_NEG2) != 0) != dneg;
+      u32 ent[2 * N];
+      ks_load_entry<2 * N>(ent, tab + (((size_t)w << (W - 1)) + idx) * 2 * N);
+      aff P;
+      P.x = load_fe_n<N>(ent);
+      P.y = load_fe_n<N>(ent + N);
+      P.y = F::cmov(P.y, F::neg(P.y), neg);
+      if (w == windows - 1) acc = W_::from_aff(P);
+      else acc = W_::madd(acc, P);
+    }
+    return acc;
+  }
+  // acc + u1*G, as SW<C>::dsm
+  static EB_HD jac g_part(jac acc, size_t i, size_t cnt_items, u32 flags, const u32* ws, const u32* gtab) {
+    for (int j = 0; j < W_::GWINDOWS; j++) {
+      bool dneg;
+      u32 idx = ks_digit(W_::extract(ws, cnt_items, i, 0, W_::GW * j, W_::GW), j == W_::GWINDOWS - 1, W_::GW, &dneg);
+      bool neg = dneg != ((flags & W_::FL_NEGG) != 0);
+      const u32* ent = gtab + ((size_t)j * W_::GENTRIES + idx) * 2 * N;
+      aff P;
+      P.x = load_fe_n<N>(ent);
+      P.y = load_fe_n<N>(ent + N);
+      P.y = F::cmov(P.y, F::neg(P.y), neg);
+      acc = W_::madd(acc, P);
+    }
+    return acc;
+  }
+
   static EB_HD uint8_t verify_keyed_item(size_t i, size_t cnt_items, const u32* key_idx, const uint8_t* kst, int W,
                                          int windows, const u32* ktab, const uint8_t* r, const u32* ws, const u32* gtab) {
     const size_t LEN = C::LEN;
@@ -286,6 +433,68 @@ struct SWKeyed {
       if (F::eq(acc.x, F::mul(F::to_mont(rn), z2))) return 1;
     }
     return 0;
+  }
+  // k256_mul_keyed_item on this curve: Jacobian result word-major (coordinate c, word w at jout[(N c + w) cnt + i]),
+  // Montgomery form; 1 = ST_TRUE, 4 = ST_NEEDS_HOST, or the key's throw.
+  static EB_HD uint8_t mul_keyed_item(size_t i, size_t cnt_items, const u32* key_idx, const uint8_t* kst, int W, int windows,
+                                      const u32* ktab, const u32* ws, const u32* gtab, u32* jout) {
+    const u32 k = key_idx[i];
+    const uint8_t ks = kst[k];
+    jac acc = W_::infinity();
+    if (ks == 1) {
+      u32 flags = ws[(size_t)(2 * N) * cnt_items + i];
+      acc = key_part(i, cnt_items, flags, W, windows, ktab + ((size_t)k * windows << (W - 1)) * 2 * N, ws);
+      if (!(flags & W_::FL_NOG)) acc = g_part(acc, i, cnt_items, flags, ws, gtab);
+    }
+    for (int w = 0; w < N; w++) {
+      jout[(size_t)w * cnt_items + i] = acc.x.v[w];
+      jout[(size_t)(N + w) * cnt_items + i] = acc.y.v[w];
+      jout[(size_t)(2 * N + w) * cnt_items + i] = acc.z.v[w];
+    }
+    return ks == 1 ? 1 : ks == 0 ? 4 : ks;
+  }
+
+  // k256_ks_norm_thread on this curve: LEN bytes x (xonly) or x || y per item, as SW<C>::store_point writes them.
+  // scratch: N x cnt_items words.
+  static EB_HD void norm_thread(size_t tid, size_t T, size_t cnt_items, const u32* jac_in, u32* scratch, bool xonly,
+                                uint8_t* out, uint8_t* status) {
+    const size_t LEN = C::LEN, ob = xonly ? LEN : 2 * LEN;
+    fe prod = F::one();
+    u32 live = 0;
+    int cnt = 0;
+    for (int j = 0; j < W_::BATCH; j++) {
+      size_t i = tid + (size_t)j * T;
+      if (i >= cnt_items) break;
+      cnt = j + 1;
+      fe z = load_soa(jac_in, 2, cnt_items, i);
+      if (status[i] != 1 || F::is_zero(z)) continue;
+      live |= 1u << j;
+      for (int w = 0; w < N; w++) scratch[(size_t)w * cnt_items + i] = prod.v[w];
+      prod = F::mul(prod, z);
+    }
+    if (cnt == 0) return;
+    fe inv = F::inv(prod);
+    for (int j = cnt - 1; j >= 0; j--) {
+      size_t i = tid + (size_t)j * T;
+      uint8_t* o = out + ob * i;
+      if (!((live >> j) & 1)) {
+        for (size_t b = 0; b < ob; b++) o[b] = 0;
+        if (status[i] == 1) status[i] = 7;               // ST_INFINITY
+        continue;
+      }
+      fe pre;
+      for (int w = 0; w < N; w++) pre.v[w] = scratch[(size_t)w * cnt_items + i];
+      fe zi = F::mul(inv, pre);                          // Z_i^-1
+      inv = F::mul(inv, load_soa(jac_in, 2, cnt_items, i));
+      fe zi2 = F::sqr(zi);
+      W_::stb(o, F::from_mont(F::mul(load_soa(jac_in, 0, cnt_items, i), zi2)).v);
+      if (!xonly) W_::stb(o + LEN, F::from_mont(F::mul(F::mul(load_soa(jac_in, 1, cnt_items, i), zi2), zi)).v);
+    }
+  }
+  static EB_HD fe load_soa(const u32* jac_in, int c, size_t cnt_items, size_t i) {
+    fe r;
+    for (int w = 0; w < N; w++) r.v[w] = jac_in[(size_t)(c * N + w) * cnt_items + i];
+    return r;
   }
 };
 

@@ -1,4 +1,4 @@
-// keyset.h -- the key-set kernels (keyset.cu), launched by eb200.cu
+// keyset.h -- the key-set kernels (keyset.cu, keyset_mul.cu, eddsa_keyset.cu), launched by eb200.cu
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -34,6 +34,28 @@ struct KeyedVerifyArgs {
 // adds the kernels launched (two) to *launches.  Other curve ids launch nothing and return cudaErrorInvalidValue.
 cudaError_t keyset_verify_launch(int curve, size_t n, const KeysetDev& k, const KeyedVerifyArgs& a, cudaStream_t st,
                                  cudaEvent_t main_begin, cudaEvent_t main_end, unsigned* launches);
+
+// keyset_mul.cu.  Device buffers of one keyed mul / mulAdd / derive block: k1 (NULL: no base-point term), k2 (n x len, as the caller
+// gave them: the replay uses them unreduced) and key_idx in; ws as the curve's unkeyed prep_scalars kernel left it;
+// jac: 3 x limbs x n words and scratch: limbs x n words of workspace; out (n x 2 len, or n x len for derive) and status
+// out.  batch: items per normalisation thread on secp256k1 (the other curves use SW<C>::BATCH).
+struct KeyedMulArgs {
+  const uint8_t *k1, *k2;
+  const uint32_t* key_idx;
+  const uint32_t* ws;
+  uint32_t *jac, *scratch;
+  const uint32_t *gtab, *replay_tab;
+  uint8_t *out, *status;
+  int batch;
+  bool derive;
+};
+
+// Launches the keyed main kernel (between main_begin and main_end), the normalisation and, unless a.derive, the keyed
+// replay of off-curve-key items on `st`; adds the kernels launched (three, or two for derive) to *launches.  For
+// derive, the off-curve-key items are left as ST_NEEDS_HOST with zeroed output.  Other curve ids launch nothing and
+// return cudaErrorInvalidValue.
+cudaError_t keyset_mul_launch(int curve, size_t n, const KeysetDev& k, const KeyedMulArgs& a, cudaStream_t st,
+                              cudaEvent_t main_begin, cudaEvent_t main_end, unsigned* launches);
 
 // ed25519 (eddsa_keyset.cu).  Build: classifies the m raw keys in k.xy and builds their tables on `st`; bases: scratch of
 // m * ed_keyset_windows(W) * 24 words.  Adds the kernels launched (three) to *launches.

@@ -727,6 +727,34 @@ class KeySet(_NativeSets):
             raise
         self.table_bits = self.table_bits[0] if len(set(self.table_bits)) == 1 else tuple(self.table_bits)
 
+    def _keyed(self, fn, ins, key_idx, outs):
+        """fn(set, n, *ins, key_idx, *outs) for the items of each native set: ins and outs are arrays with one row per
+        item (None passes NULL); a set that holds one native set per wire format gets its items split by `_where`."""
+        key_idx = np.asarray(key_idx)
+        n = len(key_idx)
+        if n and (key_idx.min() < 0 or key_idx.max() >= len(self.status)):
+            raise ValueError("key_idx out of range")
+        if not self._sets and n:
+            raise EllipticError("key set is closed")
+        if len(self._sets) == 1:
+            nat.call(fn, self._sets[0], n, *ins, np.ascontiguousarray(key_idx, np.uint32), *outs)
+            return
+        where = self._where[key_idx]
+        for k, h in enumerate(self._sets):
+            sel = np.nonzero(where[:, 0] == k)[0]
+            if len(sel):
+                part = [np.empty((len(sel),) + o.shape[1:], o.dtype) for o in outs]
+                nat.call(fn, h, len(sel), *(None if a is None else np.ascontiguousarray(a[sel]) for a in ins),
+                         np.ascontiguousarray(where[sel, 1]), *part)
+                for o, p in zip(outs, part):
+                    o[sel] = p
+
+    def _packed_scalars(self, name, ks, n):
+        ks = [np.ascontiguousarray(a, dtype=np.uint8) for a in ks]
+        if any(a.shape != (n, self._ec._len) for a in ks):
+            raise ValueError("%s: scalars must be (n, %d) uint8 arrays, n = len(key_idx)" % (name, self._ec._len))
+        return ks
+
     def verify_batch_packed(self, e, r, s, key_idx):
         """e, r, s: (n, len) uint8 arrays (big-endian); key_idx: n indices into the set.  Returns the status bytes."""
         lib = nat.load()
@@ -736,23 +764,67 @@ class KeySet(_NativeSets):
         n = e.shape[0]
         if not (e.shape == (n, ln) and r.shape == e.shape and s.shape == e.shape and key_idx.shape == (n,)):
             raise ValueError("e, r, s must be (n, %d) uint8 arrays and key_idx (n,)" % ln)
-        if n and (key_idx.min() < 0 or key_idx.max() >= len(self.status)):
-            raise ValueError("key_idx out of range")
-        if not self._sets and n:
-            raise EllipticError("key set is closed")
         status = np.empty(n, np.uint8)
-        if len(self._sets) == 1:
-            nat.call(lib.eb200_ecdsa_verify_batch_keyed, self._sets[0], n, e, r, s, np.ascontiguousarray(key_idx, np.uint32), status)
-            return status
-        where = self._where[key_idx]
-        for k, h in enumerate(self._sets):
-            sel = np.nonzero(where[:, 0] == k)[0]
-            if len(sel):
-                st = np.empty(len(sel), np.uint8)
-                nat.call(lib.eb200_ecdsa_verify_batch_keyed, h, len(sel), np.ascontiguousarray(e[sel]), np.ascontiguousarray(r[sel]),
-                         np.ascontiguousarray(s[sel]), np.ascontiguousarray(where[sel, 1]), st)
-                status[sel] = st
+        self._keyed(lib.eb200_ecdsa_verify_batch_keyed, (e, r, s), key_idx, (status,))
         return status
+
+    def mul_batch_packed(self, k, key_idx):
+        """pub.mul(k) for key key_idx[i] of the set (eb200_scalar_mul_batch_keyed): k is an (n, len) uint8 array, any
+        value below 2^(8 len).  Returns ((n, 2 len) x || y big-endian, statuses) as EC.mul_batch's call leaves them."""
+        key_idx = np.asarray(key_idx)
+        n = len(key_idx)
+        (k,) = self._packed_scalars("mul_batch_packed", (k,), n)
+        out, st = np.empty((n, 2 * self._ec._len), np.uint8), np.empty(n, np.uint8)
+        self._keyed(nat.load().eb200_scalar_mul_batch_keyed, (k,), key_idx, (out, st))
+        return out, st
+
+    def mul_add_batch_packed(self, k1, k2, key_idx):
+        """G.mulAdd(k1, pub, k2) for key key_idx[i] (eb200_mul_add_batch_keyed); as mul_batch_packed."""
+        key_idx = np.asarray(key_idx)
+        n = len(key_idx)
+        k1, k2 = self._packed_scalars("mul_add_batch_packed", (k1, k2), n)
+        out, st = np.empty((n, 2 * self._ec._len), np.uint8), np.empty(n, np.uint8)
+        self._keyed(nat.load().eb200_mul_add_batch_keyed, (k1, k2), key_idx, (out, st))
+        return out, st
+
+    def derive_batch_packed(self, priv, key_idx):
+        """keyPair.derive(pub) for key key_idx[i] (eb200_ecdh_derive_batch_keyed): priv is an (n, len) uint8 array.
+        Returns ((n, len) shared x big-endian, statuses)."""
+        key_idx = np.asarray(key_idx)
+        n = len(key_idx)
+        (priv,) = self._packed_scalars("derive_batch_packed", (priv,), n)
+        out, st = np.empty((n, self._ec._len), np.uint8), np.empty(n, np.uint8)
+        self._keyed(nat.load().eb200_ecdh_derive_batch_keyed, (priv,), key_idx, (out, st))
+        return out, st
+
+    def _check_imported(self, key_idx):
+        """Raise the reference's error for the first item whose key threw at import, as keyFromPublic would."""
+        key_idx = np.asarray(key_idx, np.int64)
+        if len(key_idx) and (key_idx.min() < 0 or key_idx.max() >= len(self.status)):
+            raise ValueError("key_idx out of range")
+        ks = self.status[key_idx]
+        bad = np.flatnonzero(ks > nat.ST_TRUE)
+        if len(bad):
+            raise EllipticError(_THROW_MSG.get(int(ks[bad[0]]), "status %d" % int(ks[bad[0]])))
+
+    def mul_batch(self, key_idx, ks):
+        """[pub.mul(k)] for pub = key key_idx[i]: what EC.mul_batch returns for those points, (x, y) or None = infinity."""
+        self._check_imported(key_idx)
+        out, st = self.mul_batch_packed(self._ec._scalars(ks), key_idx)
+        return _unpack(out, self._ec._len, st)
+
+    def mul_add_batch(self, k1s, key_idx, k2s):
+        """[G.mulAdd(k1, pub, k2)] for pub = key key_idx[i]: what EC.mul_add_batch returns."""
+        self._check_imported(key_idx)
+        out, st = self.mul_add_batch_packed(self._ec._scalars(k1s), self._ec._scalars(k2s), key_idx)
+        return _unpack(out, self._ec._len, st)
+
+    def derive_batch(self, privs, key_idx):
+        """[keyPair(priv).derive(pub)] for pub = key key_idx[i]: what EC.derive_batch returns, (values, statuses)."""
+        self._check_imported(key_idx)
+        ec = self._ec
+        out, st = self.derive_batch_packed(ec._scalars([_bn(p) % ec.n for p in privs]), key_idx)
+        return _unpack(out, ec._len, st), st
 
     def verify_batch(self, msgs, sigs, key_idx, enc=None, msg_bit_length=None):
         """Lists of the reference's message and signature forms, as EC.verify_batch takes them; `enc` is accepted for

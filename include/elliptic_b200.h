@@ -305,6 +305,29 @@ int eb200_keyset_destroy(eb200_keyset* ks);          /* NULL is a no-op returnin
 int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r,
                                    const uint8_t* s, const uint32_t* key_idx, uint8_t* status);
 
+/* Point.mul / G.mulAdd / KeyPair.derive against the keys of a set (`pub = key.getPublic(); pub.precompute()` once, then
+ * `pub.mul(k)`, `G.mulAdd(k1, pub, k2)`, `keyPair.derive(pub)` many times; curve/short.js:422-441, ec/key.js:102-107):
+ * item i uses key key_idx[i].  For a key that imported (key_status TRUE or FALSE), out and status[i] are byte for byte
+ * what eb200_scalar_mul_batch / eb200_mul_add_batch / eb200_ecdh_derive_batch write for the same scalars with the point
+ * = that key's decoded x || y; for a key whose import threw, status[i] is that throw and the output is zeroed.  Scalars
+ * are any value below 2^(8 len), as in the unkeyed calls (an on-curve key reduces them mod n; k = 0 mod n gives
+ * INFINITY).  An off-curve key (an {x, y} or uncompressed key is not validated) follows the UNKEYED call: mul / mulAdd
+ * replay the unkeyed call's schedule for an arbitrary point on the key's coordinates, derive is THROW_NOT_VALIDATED.
+ * That is not the reference's _fixedNafMul schedule for a precomputed point, whose answer for an off-curve point
+ * differs; eb200_ecdsa_verify_batch_keyed follows the same convention.
+ * An EdDSA set, a key_idx[i] >= m or a NULL pointer: EB200_ERR_ARG; a set whose devices eb200_shutdown released:
+ * EB200_ERR_NOT_INIT; both before anything is written.  n = 0: EB200_OK.  Host pointers, sharded over the set's devices
+ * and chunked with copy / compute overlap as eb200_ecdsa_verify_batch_keyed.  derive clears the private scalars, their
+ * digit words and the Jacobian results from the library's device buffers before it returns.
+ * eb200_last_timing: main_kernel_ms = the keyed main kernel; launches = 4 per chunk (scalar prep, keyed main, batched
+ * normalisation to affine, then the keyed replay of off-curve-key items, or for derive the status map). */
+int eb200_scalar_mul_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* k, const uint32_t* key_idx, uint8_t* out_xy,
+                                 uint8_t* status);
+int eb200_mul_add_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* k1, const uint8_t* k2, const uint32_t* key_idx,
+                              uint8_t* out_xy, uint8_t* status);
+int eb200_ecdh_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* priv, const uint32_t* key_idx, uint8_t* out_x,
+                                  uint8_t* status);
+
 /* EdDSA key sets: `key = eddsa.keyFromPublic(bytes)` once, then `eddsa.verify(msg, sig, key)` many times
  * (lib/elliptic/eddsa/index.js:52-63, eddsa/key.js:17-44), on ed25519.  The handle is the same eb200_keyset: _info
  * reports EB200_CURVE_ED25519, _destroy and eb200_shutdown treat it as any other set, and passing it to
