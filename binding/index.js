@@ -403,21 +403,25 @@ Short.validateBatch = function validateBatch(ps) {
     Uint8Array.from(be(this.b.fromRed(), len)), null, pack(ps, 2 * len, xy(len)), null, null, 1);
   return Array.prototype.map.call(res.status, function(v) { return v === 1; });
 };
-// curve.edwards#mulBatch / mulAddBatch on the ed25519 preset (edwards.js:362-375)
+// curve.edwards#mulBatch / mulAddBatch on the ed25519 preset (edwards.js:362-375).  The group has order 8n (cofactor 8):
+// a point's scalar is reduced mod 8n, which keeps k P for points with a torsion component; G's scalar mod n.
 var Edw = elliptic.curve.edwards.prototype;
 Edw.mulBatch = function mulBatch(points, ks) {
   var self = this;
   if (presetName(this) !== 'ed25519') return ks.map(function(k, i) { return (points ? points[i] : self.g).mul(new BN(k, 16)); });
   init();
-  var k = pack(ks, 32, function(v) { return be(new BN(v, 16).umod(self.n), 32); });
+  var n8 = this.n.muln(8);
+  var k = pack(ks, 32, function(v) { return be(new BN(v, 16).umod(n8), 32); });
   return pointsOut(this, native.mulAddBatch(CURVE.ed25519, null, k, points && pack(points, 64, xy(32))), ks.length, 32);
 };
 Edw.mulAddBatch = function mulAddBatch(k1s, p2s, k2s) {
   var self = this;
   if (presetName(this) !== 'ed25519') return k1s.map(function(k, i) { return self.g.mulAdd(new BN(k, 16), p2s[i], new BN(k2s[i], 16)); });
   init();
+  var n8 = this.n.muln(8);
   var f = function(v) { return be(new BN(v, 16).umod(self.n), 32); };
-  return pointsOut(this, native.mulAddBatch(CURVE.ed25519, pack(k1s, 32, f), pack(k2s, 32, f), pack(p2s, 64, xy(32))), k1s.length, 32);
+  var f8 = function(v) { return be(new BN(v, 16).umod(n8), 32); };
+  return pointsOut(this, native.mulAddBatch(CURVE.ed25519, pack(k1s, 32, f), pack(k2s, 32, f8), pack(p2s, 64, xy(32))), k1s.length, 32);
 };
 // curve.mont#mulBatch on curve25519: x-only points (mont.js:130-153); mulAdd throws in the reference and is left alone
 elliptic.curve.mont.prototype.mulBatch = function mulBatch(points, ks) {

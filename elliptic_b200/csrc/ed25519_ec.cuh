@@ -95,9 +95,12 @@ EB_HD ed_ext ed_add_mul_base(ed_ext acc, const u32* s, const u32* gtab) {
   }
   return acc;
 }
-// k * P for an on-curve affine P and k < 2^253 (little-endian limbs): 64 signed 4-bit windows over the per-item
-// cached table {0..8} P in `tab` (ED_ATAB_WORDS words)
+// k * P for an on-curve affine P (k: little-endian limbs): signed 4-bit windows over the per-item cached table
+// {0..8} P in `tab` (ED_ATAB_WORDS words).  WINDOWS = 64 covers k < 2^253 (verify's u2 < n); WINDOWS = 65 covers any
+// 256-bit k, the extra top window taking the carry out of the recoding (a digit of 0 or 1).
+template <int WINDOWS>
 EB_HD ed_ext ed_mul_var(const u32* k, const f25& px, const f25& py, u32* tab) {
+  static_assert(WINDOWS == 64 || WINDOWS == 65, "ed_mul_var: 64 or 65 windows");
   {
     ed_ext p; p.x = px; p.y = py; p.z = f25_one(); p.t = f25_mul(px, py);
     ed_cached c1 = ed_to_cached(p);
@@ -109,14 +112,20 @@ EB_HD ed_ext ed_mul_var(const u32* k, const f25& px, const f25& py, u32* tab) {
       if (m < 8) acc = ed_add_cached(acc, c1);
     }
   }
-  u32 h[8];
+  u32 h[8], top;
   {
     const u32 off[8] = {0x88888888u, 0x88888888u, 0x88888888u, 0x88888888u, 0x88888888u, 0x88888888u, 0x88888888u, 0x88888888u};
-    add_n<8>(h, k, off);
+    top = add_n<8>(h, k, off);
   }
   ed_ext acc = ed_identity();
+  if constexpr (WINDOWS == 65) {
+    ed_cached c;
+    c.ypx = f25_load(tab + 32 * top); c.ymx = f25_load(tab + 32 * top + 8);
+    c.z = f25_load(tab + 32 * top + 16); c.t2d = f25_load(tab + 32 * top + 24);
+    acc = ed_add_cached(acc, c);
+  }
   for (int w = 63; w >= 0; w--) {
-    if (w != 63)
+    if (WINDOWS == 65 || w != 63)
       for (int d = 0; d < 4; d++) acc = ed_dbl(acc);
     u32 word = 0;
 #pragma unroll
@@ -157,7 +166,7 @@ EB_HD uint8_t ed_ec_verify_item(size_t i, const uint8_t* e, const uint8_t* r, co
   EdS::fe sinv = EdS::inv(EdS::to_mont(sm));
   EdS::fe u1 = EdS::from_mont(EdS::mul(EdS::to_mont(em), sinv));  // e s^-1 mod n
   EdS::fe u2 = EdS::from_mont(EdS::mul(EdS::to_mont(rm), sinv));  // r s^-1 mod n
-  ed_ext acc = ed_mul_var(u2.v, qx, qy, atab + (size_t)i * ED_ATAB_WORDS);
+  ed_ext acc = ed_mul_var<64>(u2.v, qx, qy, atab + (size_t)i * ED_ATAB_WORDS);
   acc = ed_add_mul_base(acc, u1.v, gtab);
   // p.isInfinity(): x == 0 && y == z  (edwards.js:167-172)
   if (f25_is_zero(acc.x) && f25_eq(acc.y, acc.z)) return ST_FALSE;
@@ -264,21 +273,26 @@ EB_HD uint8_t ed_ec_keygen_item(size_t i, const uint8_t* entropy, int ne, const 
 }
 
 // Point.mul / Point.mulAdd (edwards.js:362-375) and KeyPair.derive (ec/key.js:102-107) on ed25519:
-// k1 == NULL: k2 * P;  pts == NULL: k2 * G;  both: k1 * G + k2 * P.  Scalars: 32 B big-endian, reduced mod n.
+// k1 == NULL: k2 * P;  pts == NULL: k2 * G;  both: k1 * G + k2 * P.  Scalars: 32 B big-endian.  The reference uses k as
+// given and the group has order 8n (cofactor 8), so P's scalar runs over all its 256 bits: reducing it mod n would
+// change k2 * P whenever P has a torsion component.  G has order n and its scalars are reduced mod n; so is the
+// private key of derive, as _importPrivate (ec/key.js:76-82) holds it.
 // out: x || y big-endian (the neutral element is the ordinary point (0, 1)).  derive: x only semantics are
 // applied by the host wrapper; an off-curve P is status 3 ('public point not validated') there, 4 otherwise.
 EB_HD uint8_t ed_ec_mul_add_item(size_t i, const uint8_t* k1, const uint8_t* k2, const uint8_t* pts, bool derive,
                                  const u32* gtab, u32* atab, uint8_t* out) {
   for (int b = 0; b < 64; b++) out[64 * i + b] = 0;
   u32 s1[8], s2[8];
-  ed_scalar_mod_n(s2, k2 + 32 * i);
   ed_ext acc = ed_identity();
   if (pts) {
     f25 px = f25_from_be(pts + 64 * i), py = f25_from_be(pts + 64 * i + 32);
     if (!ed_on_curve(px, py)) return derive ? ST_THROW_NOT_VALIDATED : ST_NEEDS_HOST;
-    acc = ed_mul_var(s2, px, py, atab + (size_t)i * ED_ATAB_WORDS);
+    if (derive) ed_scalar_mod_n(s2, k2 + 32 * i);
+    else load_be<8>(s2, k2 + 32 * i);
+    acc = ed_mul_var<65>(s2, px, py, atab + (size_t)i * ED_ATAB_WORDS);
     if (k1) { ed_scalar_mod_n(s1, k1 + 32 * i); acc = ed_add_mul_base(acc, s1, gtab); }
   } else {
+    ed_scalar_mod_n(s2, k2 + 32 * i);
     acc = ed_add_mul_base(acc, s2, gtab);
   }
   f25 zi = f25_inv(acc.z);

@@ -539,12 +539,14 @@ class EC(_KeyObjects):
 
     # ---- curve.point(...).mul / mulAdd batches (short.js:422-441) ---------------------------------------------
     def _scalars(self, ks):
+        # k P == (k mod order) P for every on-curve P: the group has order n on the short curves, 8n on ed25519 (cofactor 8)
+        order = 8 * self.n if self.name == "ed25519" else self.n
         vals = []
         for k in ks:
             k = _bn(k)
             if k < 0:
                 raise EllipticError("negative scalars are not supported by the batch path")
-            vals.append(k % self.n if k >> (8 * self._len) else k)          # same point for every on-curve input
+            vals.append(k % order if k >> (8 * self._len) else k)
         return _pack(vals, self._len)
 
     def _points(self, pts):

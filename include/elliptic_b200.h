@@ -224,7 +224,9 @@ int eb200_ec_keygen_batch(int curve, size_t n, const uint8_t* entropy, size_t en
  *  - EB200_CURVE_ED25519 is accepted by eb200_ecdsa_verify_batch (+ _der, SEC1 formats: BaseCurve.decodePoint and
  *    EdwardsCurve.pointFromX, edwards.js:46-69), eb200_ecdsa_sign_batch (+ _k, _pers), eb200_ec_keygen_batch,
  *    eb200_scalar_mul_batch / eb200_mul_add_batch (Point.mul / mulAdd, edwards.js:362-375; 32-byte big-endian x || y,
- *    the neutral element is the ordinary point (0, 1)) and eb200_ecdh_derive_batch: new elliptic.ec('ed25519')
+ *    the neutral element is the ordinary point (0, 1); the point's scalar is used as given, any value below 2^256, so
+ *    that k P is exact for points with a torsion component too (the group has order 8n), and G's scalar is reduced
+ *    mod n) and eb200_ecdh_derive_batch: new elliptic.ec('ed25519')
  *    (test/ecdsa-test.js:130, test/ecdh-test.js:26; eqXToP edwards.js:415-431).  An un-validated off-curve point is
  *    reported as EB200_ST_NEEDS_HOST (the reference's answer then depends on its own wNAF schedule, which is not
  *    replayed for this curve); eb200_ecdsa_recover_batch returns EB200_ERR_UNSUPPORTED.

@@ -104,9 +104,9 @@ def test_curve_api_mul_mul_add_and_ecdh(native):
     mul = gec.mul_batch(pts, k2)
     for i in range(0, n, 2):
         P = ec.curve.point(pts[i][0], pts[i][1])
-        w = ec.g.mul_add(k1[i] % ec.n, P, k2[i] % ec.n)
+        w = ec.g.mul_add(k1[i], P, k2[i])
         assert got[i] == (w.get_x(), w.get_y())
-        w = P.mul(k2[i] % ec.n)
+        w = P.mul(k2[i])
         assert mul[i] == (w.get_x(), w.get_y())
     assert mul[0] == (0, 1) and mul[1] == (0, 1)                     # the neutral element is an ordinary point
     # ECDH (test/ecdh-test.js:26): both sides agree, and equal the oracle
