@@ -464,6 +464,40 @@ static napi_value EddsaVerifyBatchKeyed(napi_env env, napi_callback_info info) {
   return rc ? fail(env, rc) : arr;
 }
 
+/* eddsaSigningSetCreate(secrets: m x 32) -> {handle, pub: Uint8Array(32 m)}   (eddsa.keyFromSecret for m keys) */
+static napi_value EddsaSigningSetCreate(napi_env env, napi_callback_info info) {
+  ARGS(1); BUF(0, sec, ls);
+  size_t m = ls / 32;
+  if (ls % 32) return fail(env, EB200_ERR_ARG);
+  keyset_box* b = (keyset_box*)calloc(1, sizeof *b);
+  if (!b) return fail(env, EB200_ERR_ARG);
+  uint8_t* pub; napi_value apub = out_u8(env, 32 * m, &pub);
+  int rc = eb200_eddsa_signing_set_create(m, sec, pub, &b->ks);
+  if (rc) { free(b); return fail(env, rc); }
+  napi_value o = obj(env), h;
+  napi_create_external(env, b, keyset_finalize, 0, &h);
+  SET(o, "handle", h); SET(o, "pub", apub);
+  return o;
+}
+/* eddsaSignBatchKeyed(handle, msgs | null, msgOff, keyIdx: Uint8Array over n little-endian uint32) -> Uint8Array(64 n)
+ * of signatures Rencoded || S   (key.sign(msg) for keys of a signing set) */
+static napi_value EddsaSignBatchKeyed(napi_env env, napi_callback_info info) {
+  ARGS(4); OPT(1, msgs, lm); BUF(2, off, lo); BUF(3, idx, li);
+  void* p = 0;
+  if (napi_get_value_external(env, argv[0], &p) != napi_ok || !p || !((keyset_box*)p)->ks) return fail(env, EB200_ERR_ARG);
+  eb200_keyset* ks = ((keyset_box*)p)->ks;
+  size_t n = li / 4;
+  if (li != 4 * n || ((uintptr_t)idx & 3) || lo != 8 * (n + 1) || ((uintptr_t)off & 7)) return fail(env, EB200_ERR_ARG);
+  const uint64_t* o = (const uint64_t*)off;
+  for (size_t i = 0; i < n; i++) if (o[i + 1] < o[i]) return fail(env, EB200_ERR_ARG);
+  if (o[n] > lm) return fail(env, EB200_ERR_ARG);
+  uint8_t *sig, *st;
+  napi_value asig = out_u8(env, 64 * n, &sig);
+  out_u8(env, n, &st);                                                 /* always EB200_ST_TRUE */
+  int rc = eb200_eddsa_sign_batch_keyed(ks, n, msgs, o, (const uint32_t*)(const void*)idx, sig, st);
+  return rc ? fail(env, rc) : asig;
+}
+
 static napi_value Register(napi_env env, napi_value exports) {
   static const struct { const char* name; napi_callback cb; } fns[] = {
       {"init", Init}, {"ecdsaVerifyBatch", EcdsaVerifyBatch}, {"ecdsaVerifyBatchAsync", EcdsaVerifyBatchAsync},
@@ -474,7 +508,8 @@ static napi_value Register(napi_env env, napi_value exports) {
       {"x25519Batch", X25519Batch},
       {"keysetCreate", KeysetCreate}, {"keysetDestroy", KeysetDestroy}, {"ecdsaVerifyBatchKeyed", EcdsaVerifyBatchKeyed},
       {"eddsaKeysetCreate", EddsaKeysetCreate}, {"eddsaVerifyBatchKeyed", EddsaVerifyBatchKeyed},
-      {"mulAddBatchKeyed", MulAddBatchKeyed}, {"ecdhDeriveBatchKeyed", EcdhDeriveBatchKeyed}};
+      {"mulAddBatchKeyed", MulAddBatchKeyed}, {"ecdhDeriveBatchKeyed", EcdhDeriveBatchKeyed},
+      {"eddsaSigningSetCreate", EddsaSigningSetCreate}, {"eddsaSignBatchKeyed", EddsaSignBatchKeyed}};
   for (unsigned i = 0; i < sizeof fns / sizeof fns[0]; i++) {
     napi_value f;
     napi_create_function(env, fns[i].name, NAPI_AUTO_LENGTH, fns[i].cb, 0, &f);

@@ -4,7 +4,7 @@
 // run on the GPU through the N-API addon -> libelliptic_b200.so (include/elliptic_b200.h):
 //   EC#verifyBatch / verifyBatchAsync / signBatch / genKeyPairBatch / recoverPubKeyBatch / getKeyRecoveryParamBatch /
 //   deriveBatch
-//   EDDSA#verifyBatch / signBatch / keySet
+//   EDDSA#verifyBatch / signBatch / keySet / signingSet
 //   curve.short#mulBatch / mulAddBatch / addBatch / dblBatch / validateBatch   (any parameters, presets take the tuned kernels)
 //   curve.edwards#mulBatch / mulAddBatch (ed25519), curve.mont#mulBatch (curve25519)
 // All parsing (hex / byte arrays / DER / SEC1, _truncateToN) is done by the reference's own JS, so accept / reject /
@@ -332,6 +332,32 @@ elliptic.eddsa.prototype.keySet = function keySet(pubs) {
       var m = concatMsgs(ms);
       return Array.prototype.map.call(native.eddsaVerifyBatchKeyed(set.handle, R, S, null, m.blob, m.off, new Uint8Array(idx.buffer)),
         statusToBool);
+    },
+    destroy: function() { native.keysetDestroy(set.handle); }
+  };
+};
+// EDDSA#signingSet(secrets) -> {pub, signBatch(messages, keyIdx), destroy()}: the batch form of
+// `key = eddsa.keyFromSecret(secret)` once and key.sign(msg) many times.  The GPU keeps each key's clamped scalar, message
+// prefix and encoded public key (pub: key.getPublic('bytes') per key), not the secret; signBatch returns Signature objects.
+elliptic.eddsa.prototype.signingSet = function signingSet(secrets) {
+  var self = this;
+  var secs = secrets.map(function(s) { return elliptic.utils.parseBytes(s); });
+  if (secs.some(function(s) { return s.length !== 32; })) throw new Error('signing sets take 32-byte secrets');
+  init();
+  var set = native.eddsaSigningSetCreate(pack(secs, 32, function(s) { return s; }));
+  var pubs = [];
+  for (var k = 0; k < secs.length; k++) pubs.push(Array.from(set.pub.subarray(32 * k, 32 * k + 32)));
+  return {
+    pub: pubs,
+    signBatch: function(messages, keyIdx) {
+      var n = messages.length, idx = new Uint32Array(n);
+      for (var i = 0; i < n; i++) {
+        if (!(keyIdx[i] >= 0 && keyIdx[i] < pubs.length)) throw new Error('key index out of range');
+        idx[i] = keyIdx[i];
+      }
+      var m = concatMsgs(messages.map(function(x) { return elliptic.utils.parseBytes(x); }));
+      var sig = native.eddsaSignBatchKeyed(set.handle, m.blob, m.off, new Uint8Array(idx.buffer));
+      return messages.map(function(_, i) { return self.makeSignature(Array.from(sig.subarray(64 * i, 64 * i + 64))); });
     },
     destroy: function() { native.keysetDestroy(set.handle); }
   };

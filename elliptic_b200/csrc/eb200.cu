@@ -2072,8 +2072,10 @@ int eb200_ecdsa_recovery_param_batch(int curve, size_t n, const uint8_t* e, cons
 // ---- key sets ---------------------------------------------------------------------------------------------------------
 // The kernels are in keyset.cu (see there why); this side owns the handles, stages the buffers and launches the unchanged
 // decode and prep kernels of this file around them.
+enum KeysetKind { KS_PUBLIC, KS_SIGNING };      // public keys (verify, mul) or ed25519 secrets (eb200_eddsa_sign_batch_keyed)
 struct eb200_keyset {
   int curve = 0;
+  int kind = KS_PUBLIC;
   size_t m = 0;
   u32 W = 0, fmt = 0;
   size_t device_bytes = 0;
@@ -2092,6 +2094,7 @@ void keyset_free_device(eb200_keyset* ks) {
   for (int i = 0; i < ks->ndev; i++) {
     KeysetDev& d = ks->dev[ks->devs[i]];
     if (cudaSetDevice(ks->devs[i]) != cudaSuccess) { cudaGetLastError(); continue; }
+    if (ks->kind == KS_SIGNING && d.tab) cudaMemset(d.tab, 0, ED_SIGNSET_KEY_BYTES * ks->m);   // the secret words
     cudaFree(d.xy); cudaFree(d.kst); cudaFree(d.tab);
     d = KeysetDev{};
   }
@@ -2327,6 +2330,66 @@ int eddsa_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* R, c
     });
 }
 
+// ---- EdDSA (ed25519) signing sets: kernels in eddsa_signset.cu -----------------------------------------------------------
+// One device's copy: secrets up, a, prefix and A derived on the GPU, A home; the staged secrets are wiped.
+int ed_signset_build_on(Ctx& c, eb200_keyset* ks, const uint8_t* secrets, uint8_t* out_pub) {
+  const size_t m = ks->m;
+  int rc = ensure_table(c, EB200_CURVE_ED25519);
+  if (rc) return rc;
+  KeysetDev& d = ks->dev[c.device];
+  CK(cudaMalloc(&d.xy, 32 * m));
+  CK(cudaMalloc(&d.tab, ED_SIGNSET_KEY_BYTES * m));
+  if ((rc = grow(&c.d_in, &c.d_in_cap, 32 * m))) return rc;
+  uint8_t* dsec = c.d_in;
+  return run_single(c, {{dsec, secrets, 32 * m}},
+    [&](Launch& L) {
+      cudaError_t err = ed_signset_create_launch(m, d, dsec, c.gtab[EB200_CURVE_ED25519], L.st, &L.count);
+      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "ed_signset_create_launch");
+    },
+    {{out_pub, d.xy, 32 * m}}, {{dsec, 32 * m}}, true);   // secrets do not stay in the shared buffer
+}
+
+// Keyed EdDSA sign of one block on one device of the set, chunked like eddsa_keyed_on (msg_off points at this block's
+// first offset, offsets absolute).  Each chunk's nonces r are cleared from the workspace behind its kernels.
+int eddsa_sign_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* msgs, const uint64_t* msg_off,
+                        const u32* key_idx, uint8_t* sig) {
+  const KeysetDev& d = ks->dev[c.device];
+  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a key pointer of another device
+  int rc = ensure_table(c, EB200_CURVE_ED25519);
+  if (rc) return rc;
+  const ChunkPlan P = make_plan(n);
+  const size_t mbytes = (size_t)(msg_off[n] - msg_off[0]);
+  const size_t off_bytes = (n + 1) * sizeof(uint64_t);
+  const size_t base = align256(n * 68);            // sig | key_idx
+  if ((rc = grow(&c.d_in, &c.d_in_cap, base + align256(off_bytes) + align256(mbytes + 1)))) return rc;
+  const size_t ws_slot = align256(ed_signset_ws_bytes(P.max_m));
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, (P.chunks > 1 ? 2 : 1) * ws_slot))) return rc;
+  uint8_t* dsig = c.d_in;
+  u32* didx = (u32*)(dsig + 64 * n);
+  uint64_t* doff = (uint64_t*)(c.d_in + base);
+  uint8_t* dm = c.d_in + base + align256(off_bytes);
+  const u32* gt = c.gtab[EB200_CURVE_ED25519];
+  return run_chunked(c, P,
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {didx + lo, key_idx + lo, 4 * m};
+      seg[1] = {doff + lo, msg_off + lo, (m + 1) * sizeof(uint64_t)};
+      seg[2] = {dm + (msg_off[lo] - msg_off[0]), msgs + msg_off[lo], (size_t)(msg_off[lo + m] - msg_off[lo])};
+      return 3;
+    },
+    [&](size_t lo, size_t m, Launch& L, int slot, int k) {
+      uint8_t* ws = c.d_ws + (size_t)slot * ws_slot;
+      cudaError_t err = ed_signset_sign_launch(m, d, dm - msg_off[0], doff + lo, didx + lo, gt, (u32*)ws, dsig + 64 * lo, L.st,
+                                               c.ev_k0[k], c.ev_k1[k], &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "ed_signset_sign_launch");
+      CK(cudaMemsetAsync(ws + ed_signset_nonce_offset(m), 0, ed_signset_nonce_bytes(m), L.st));   // the nonces r
+      return EB200_OK;
+    },
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {sig + 64 * lo, dsig + 64 * lo, 64 * m};
+      return 1;
+    });
+}
+
 // h < n for a 32-byte little-endian h (the keyed tables cover 253 bits)
 bool ed_scalar_below_n(const uint8_t* h) {
   static const uint8_t n_le[32] = {0xed, 0xd3, 0xf5, 0x5c, 0x1a, 0x63, 0x12, 0x58, 0xd6, 0x9c, 0xf7, 0xa2, 0xde, 0xf9, 0xde, 0x14,
@@ -2476,7 +2539,7 @@ int eb200_eddsa_keyset_create(size_t m, const uint8_t* A, uint32_t table_bits, u
 
 int eb200_eddsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* R, const uint8_t* S, const uint8_t* h,
                                    const uint32_t* key_idx, uint8_t* status) {
-  if (!ks || ks->curve != EB200_CURVE_ED25519) return EB200_ERR_ARG;
+  if (!ks || ks->curve != EB200_CURVE_ED25519 || ks->kind != KS_PUBLIC) return EB200_ERR_ARG;
   if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
   if (n == 0) return EB200_OK;
   if (!R || !S || !h || !key_idx || !status) return EB200_ERR_ARG;
@@ -2489,7 +2552,7 @@ int eb200_eddsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8
 int eb200_eddsa_verify_batch_keyed_msgs(const eb200_keyset* ks, size_t n, const uint8_t* R, const uint8_t* S,
                                         const uint8_t* msgs, const uint64_t* msg_off, const uint32_t* key_idx,
                                         uint8_t* status) {
-  if (!ks || ks->curve != EB200_CURVE_ED25519) return EB200_ERR_ARG;
+  if (!ks || ks->curve != EB200_CURVE_ED25519 || ks->kind != KS_PUBLIC) return EB200_ERR_ARG;
   if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
   if (n == 0) return EB200_OK;
   if (!R || !S || !msg_off || !key_idx || !status || (!msgs && msg_off[n])) return EB200_ERR_ARG;
@@ -2499,6 +2562,31 @@ int eb200_eddsa_verify_batch_keyed_msgs(const eb200_keyset* ks, size_t n, const 
   return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
     return eddsa_keyed_on(c, ks, m, R + 32 * lo, S + 32 * lo, nullptr, mp, msg_off + lo, key_idx + lo, status + lo);
   });
+}
+
+int eb200_eddsa_signing_set_create(size_t m, const uint8_t* secrets, uint8_t* out_pub, eb200_keyset** out) {
+  if (out) *out = nullptr;
+  if (!out || !secrets || m == 0 || m > 0xffffffffull) return EB200_ERR_ARG;
+  eb200_keyset* ks = new eb200_keyset;
+  ks->curve = EB200_CURVE_ED25519; ks->kind = KS_SIGNING; ks->m = m;
+  ks->device_bytes = (32 + ED_SIGNSET_KEY_BYTES) * m;
+  return keyset_create_on_devices(ks, out, [&](Ctx& c) { return ed_signset_build_on(c, ks, secrets, out_pub); });
+}
+
+int eb200_eddsa_sign_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* msgs, const uint64_t* msg_off,
+                                 const uint32_t* key_idx, uint8_t* out_sig, uint8_t* status) {
+  if (!ks || ks->curve != EB200_CURVE_ED25519 || ks->kind != KS_SIGNING) return EB200_ERR_ARG;
+  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (n == 0) return EB200_OK;
+  if (!msg_off || !key_idx || !out_sig || !status || (!msgs && msg_off[n])) return EB200_ERR_ARG;
+  for (size_t i = 0; i < n; i++) if (msg_off[i + 1] < msg_off[i] || key_idx[i] >= ks->m) return EB200_ERR_ARG;
+  static const uint8_t none = 0;
+  const uint8_t* mp = msgs ? msgs : &none;
+  int rc = run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
+    return eddsa_sign_keyed_on(c, ks, m, mp, msg_off + lo, key_idx + lo, out_sig + 64 * lo);
+  });
+  if (rc == EB200_OK) memset(status, EB200_ST_TRUE, n);         // the reference cannot fail here
+  return rc;
 }
 
 }  // extern "C"

@@ -301,15 +301,20 @@ EB_HD ed_ext ed_mul_base(const u32* s, const u32* gtab) {
   }
   return acc;
 }
-// EDDSA.encodePoint (eddsa/index.js:94-98): y little-endian, x parity in the top bit
-EB_HD void ed_encode(const ed_ext& p, uint8_t* out32) {
-  f25 zi = f25_inv(p.z);
-  f25 x = f25_normalize(f25_mul(p.x, zi)), y = f25_normalize(f25_mul(p.y, zi));
+// EDDSA.encodePoint (eddsa/index.js:94-98) of the affine point (x, y), both fully reduced (f25_normalize):
+// y little-endian, x parity in the top bit
+EB_HD void ed_encode_affine(const f25& x, const f25& y, uint8_t* out32) {
   for (int k = 0; k < 8; k++) {
     out32[4 * k] = (uint8_t)y.v[k]; out32[4 * k + 1] = (uint8_t)(y.v[k] >> 8);
     out32[4 * k + 2] = (uint8_t)(y.v[k] >> 16); out32[4 * k + 3] = (uint8_t)(y.v[k] >> 24);
   }
   out32[31] |= (x.v[0] & 1) ? 0x80 : 0;
+}
+// the same for a point in extended coordinates: one inversion
+EB_HD void ed_encode(const ed_ext& p, uint8_t* out32) {
+  f25 zi = f25_inv(p.z);
+  f25 x = f25_normalize(f25_mul(p.x, zi)), y = f25_normalize(f25_mul(p.y, zi));
+  ed_encode_affine(x, y, out32);
 }
 // 64-byte digest as a little-endian integer mod n, Montgomery form of the scalar field
 EB_HD Fp<ED25519_FN>::fe ed_digest_mod_n(const uint8_t* dg) {

@@ -1,4 +1,4 @@
-// keyset.h -- the key-set kernels (keyset.cu, keyset_mul.cu, eddsa_keyset.cu), launched by eb200.cu
+// keyset.h -- the key-set kernels (keyset.cu, keyset_mul.cu, eddsa_keyset.cu, eddsa_signset.cu), launched by eb200.cu
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -9,6 +9,8 @@
 // (a throw status, EB200_ST_TRUE = on the curve, EB200_ST_FALSE = imported but off the curve) and the tables of the
 // on-curve keys, keyset_key_bytes() apart, W bits per window.  An ed25519 set (eddsa_keyset.cu) keeps the 32 raw bytes
 // of each key in `xy`, its verdict (EB200_ST_TRUE or the decoder's throw) in `kst` and ed_keyset_key_bytes() per key.
+// An ed25519 signing set (eddsa_signset.cu) keeps each key's encoded A in `xy` and its secret words in `tab`: a
+// (Montgomery form mod n) then the 32-byte message prefix, ED_SIGNSET_KEY_BYTES per key; `kst` is NULL and W = 0.
 struct KeysetDev {
   uint8_t* xy;
   uint8_t* kst;
@@ -67,3 +69,18 @@ cudaError_t ed_keyset_gather_launch(size_t n, const KeysetDev& k, const uint32_t
 cudaError_t ed_keyset_verify_launch(size_t n, const KeysetDev& k, const uint8_t* R, const uint8_t* S, const uint8_t* h,
                                     const uint32_t* key_idx, const uint32_t* gtab, uint8_t* status, cudaStream_t st,
                                     unsigned* launches);
+
+// ed25519 signing sets (eddsa_signset.cu).  Create: secrets (m x 32) in, k.tab and k.xy (the encoded A) out; gtab: the
+// ed25519 fixed-base table.  One kernel.
+constexpr size_t ED_SIGNSET_KEY_BYTES = 64;
+cudaError_t ed_signset_create_launch(size_t m, const KeysetDev& k, const uint8_t* secrets, const uint32_t* gtab,
+                                     cudaStream_t st, unsigned* launches);
+// Workspace of a sign launch of n items, and the byte range [offset, offset + bytes) of it that holds the nonces r.
+size_t ed_signset_ws_bytes(size_t n);
+size_t ed_signset_nonce_offset(size_t n);
+size_t ed_signset_nonce_bytes(size_t n);
+// Sign: msgs / msg_off (offsets relative to msgs), key_idx in, sig (n x 64) out; ws: ed_signset_ws_bytes(n).  Launches
+// nonce (between main_begin and main_end), normalise and challenge kernels on `st` and adds three to *launches.
+cudaError_t ed_signset_sign_launch(size_t n, const KeysetDev& k, const uint8_t* msgs, const uint64_t* msg_off,
+                                   const uint32_t* key_idx, const uint32_t* gtab, uint32_t* ws, uint8_t* sig, cudaStream_t st,
+                                   cudaEvent_t main_begin, cudaEvent_t main_end, unsigned* launches);

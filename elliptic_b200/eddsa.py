@@ -29,6 +29,10 @@ class _EdKeyObjects:
         """The batch form of `key = eddsa.keyFromPublic(pub)` for many keys: an EdKeySet on the GPU."""
         return EdKeySet(self, pubs, table_bits)
 
+    def signing_set(self, secrets):
+        """The batch form of `key = eddsa.keyFromSecret(secret)` for many keys: an EdSigningSet on the GPU."""
+        return EdSigningSet(self, secrets)
+
 
 class EDDSA(_EdKeyObjects):
     def __init__(self, curve="ed25519", device=0):
@@ -233,3 +237,67 @@ class EdKeySet(_NativeSets):
         R, S, idx, _ = self._args(rs[:, :32], rs[:, 32:], key_idx)
         h = _pack([ed.hash_int(sig[i][:32], self._A[idx[i]], ms[i]) for i in range(n)], 32, "little")
         return self.verify_batch_packed(R, S, h, idx)
+
+
+class EdSigningSet(_NativeSets):
+    """ed25519 signing keys imported once from their 32-byte secrets (eb200_eddsa_signing_set_create): the GPU keeps each
+    key's clamped scalar, message prefix and encoded public key, and item i of a sign call is signed by key key_idx[i],
+    with the bytes EDDSA.sign_batch gives for that key's secret.  The object does not keep the secrets.  `public`: the
+    (m, 32) encoded public keys (key.getPublic('bytes')).  close() frees the device memory; the object is a context
+    manager."""
+
+    def __init__(self, ed, secrets):
+        self._ed = ed
+        sks = []
+        for s in secrets:
+            sk = _parse_bytes(s)
+            if len(sk) != 32:
+                raise EllipticError("unsupported secret length %d" % len(sk))
+            sks.append(sk)
+        m = len(sks)
+        sec = np.frombuffer(b"".join(sks), np.uint8).reshape(m, 32).copy()
+        lib = nat.init(ed._device)
+        self.public = np.zeros((m, 32), np.uint8)
+        h = ctypes.c_void_p()
+        try:
+            nat.check(lib.eb200_eddsa_signing_set_create(m, sec.ctypes.data, self.public.ctypes.data, ctypes.byref(h)))
+        finally:
+            sec[:] = 0
+        self._sets = [h]
+        db = ctypes.c_size_t()
+        nat.check(lib.eb200_keyset_info(h, None, None, None, ctypes.byref(db)))
+        self.device_bytes = db.value
+
+    def _handle(self):
+        if not self._sets:
+            raise EllipticError("signing set is closed")
+        return self._sets[0]
+
+    def sign_batch_packed(self, msgs, msg_off, key_idx):
+        """msgs: concatenated message bytes; msg_off: n + 1 uint64 offsets; key_idx: n indices into the set.
+        Returns the (n, 64) signatures Rencoded || S."""
+        msgs = np.ascontiguousarray(msgs, dtype=np.uint8)
+        msg_off = np.ascontiguousarray(msg_off, dtype=np.uint64)
+        key_idx = np.asarray(key_idx)
+        n = key_idx.shape[0] if key_idx.ndim == 1 else -1
+        if n < 0 or not (msg_off.shape == (n + 1,) and int(msg_off[n]) == msgs.size):
+            raise ValueError("key_idx must be (n,) and msg_off hold n + 1 offsets, the last one equal to len(msgs)")
+        if n and (key_idx.min() < 0 or key_idx.max() >= len(self.public)):
+            raise ValueError("key_idx out of range")
+        sig = np.empty((n, 64), np.uint8)
+        if n:
+            h, st = self._handle(), np.empty(n, np.uint8)
+            nat.call(nat.load().eb200_eddsa_sign_batch_keyed, h, n, msgs if msgs.size else None, msg_off,
+                     np.ascontiguousarray(key_idx, np.uint32), sig, st)
+            if not bool((st == nat.ST_TRUE).all()):
+                raise nat.NativeError("eddsa sign: unexpected status")
+        return sig
+
+    def sign_batch(self, messages, key_idx):
+        """Messages in the reference's forms (hex strings / byte arrays), as EDDSA.sign_batch takes them, each signed by
+        key key_idx[i] of the set.  Returns a list of 64-byte signatures (sig.toBytes())."""
+        n = len(messages)
+        if len(key_idx) != n:
+            raise ValueError("messages and key_idx must have the same length")
+        sig = self.sign_batch_packed(*_blob([_parse_bytes(m) for m in messages]), key_idx)
+        return [sig[i].tobytes() for i in range(n)]

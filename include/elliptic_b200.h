@@ -359,6 +359,30 @@ int eb200_eddsa_verify_batch_keyed_msgs(const eb200_keyset* ks, size_t n, const 
                                         const uint8_t* msgs, const uint64_t* msg_off, const uint32_t* key_idx,
                                         uint8_t* status);
 
+/* EdDSA signing sets: `key = eddsa.keyFromSecret(secret)` once, then `key.sign(msg)` many times (lib/elliptic/eddsa/
+ * key.js:40-75, eddsa/index.js:34-44), on ed25519.  Create runs, per key, SHA-512 of the secret, the clamp, the message
+ * prefix and A = a G, and encodes A, all on the GPU.  The set keeps a, the 32-byte prefix and the 32 bytes of A on each
+ * device, not the secret: device_bytes = 96 m.  The handle is the same eb200_keyset: _info reports EB200_CURVE_ED25519
+ * and table_bits = 0 (no table width applies), _destroy and eb200_shutdown treat it as any other set and clear its
+ * secret words before they free them.  A signing set passed to any verify / mul / derive keyed call, or a public-key
+ * set passed to eb200_eddsa_sign_batch_keyed, returns EB200_ERR_ARG.
+ *   secrets : m x 32 bytes;  out_pub : m x 32 bytes key.getPublic('bytes'), or NULL
+ * m = 0, m >= 2^32 or a NULL secrets / out: EB200_ERR_ARG; no device: EB200_ERR_NOT_INIT; a failed allocation:
+ * EB200_ERR_CUDA with *out NULL and everything freed.  The staged secrets are cleared from the library's device
+ * buffers before the call returns.  eb200_last_timing after create: launches = 1 per device. */
+int eb200_eddsa_signing_set_create(size_t m, const uint8_t* secrets, uint8_t* out_pub, eb200_keyset** out);
+/* Batch of key.sign(msg): item i is signed by key key_idx[i].  msgs / msg_off as eb200_eddsa_sign_batch takes them
+ * (msgs may be NULL when every message is empty).  out_sig: n x 64 bytes Rencoded || S, byte-identical to what
+ * eb200_eddsa_sign_batch writes with secrets[i] = that key's secret; status: n bytes, always EB200_ST_TRUE.
+ * A NULL pointer, decreasing offsets or a key_idx[i] >= m: EB200_ERR_ARG; a set whose devices eb200_shutdown released:
+ * EB200_ERR_NOT_INIT; both before anything is written.  n = 0: EB200_OK.  Host pointers, sharded over the set's
+ * devices and chunked with copy / compute overlap.  Per chunk: the nonce kernel (r = SHA512(prefix || M) mod n,
+ * R = r G), a batched normalisation of R (one inversion per 16 items) that writes Rencoded, and the challenge kernel
+ * (S = r + SHA512(Rencoded || A || M) a mod n); the nonces r are cleared from the library's workspace before the call
+ * returns.  eb200_last_timing: main_kernel_ms = the nonce kernel; launches = 3 per chunk. */
+int eb200_eddsa_sign_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* msgs, const uint64_t* msg_off,
+                                 const uint32_t* key_idx, uint8_t* out_sig, uint8_t* status);
+
 /* Self-test hooks used by the parity tests (device arithmetic vs the oracle).
  * a, b, out: n elements of L little-endian 32-bit limbs each (host pointers); L = 8, except p192 6, p384 12 and
  * p521 18.  An op the curve does not know returns a (short curves) or 0 (secp256k1, ed25519 / curve25519).
