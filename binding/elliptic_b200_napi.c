@@ -442,6 +442,24 @@ static napi_value EcdhDeriveBatchKeyed(napi_env env, napi_callback_info info) {
   return res;
 }
 
+/* ecdsaRecoveryParamBatchKeyed(handle, e, r, s, keyIdx: Uint8Array over n little-endian uint32) -> {recid, status}
+ * (getKeyRecoveryParam, ec/index.js:261-278, against key keyIdx[i]) */
+static napi_value EcdsaRecoveryParamBatchKeyed(napi_env env, napi_callback_info info) {
+  ARGS(5); BUF(1, e, le); BUF(2, r, lr); BUF(3, s, ls); BUF(4, idx, li);
+  size_t len = 0;
+  eb200_keyset* ks = ecdsa_set(env, argv[0], &len);
+  if (!ks) return fail(env, EB200_ERR_ARG);
+  size_t n = li / 4;
+  if (li != 4 * n || le != n * len || lr != le || ls != le || ((uintptr_t)idx & 3)) return fail(env, EB200_ERR_ARG);
+  uint8_t *id, *st;
+  napi_value ai = out_u8(env, n, &id), ast = out_u8(env, n, &st);
+  int rc = eb200_ecdsa_recovery_param_batch_keyed(ks, n, e, r, s, (const uint32_t*)(const void*)idx, id, st);
+  if (rc) return fail(env, rc);
+  napi_value res = obj(env);
+  SET(res, "recid", ai); SET(res, "status", ast);
+  return res;
+}
+
 /* eddsaVerifyBatchKeyed(handle, R, S, h | null, msgs | null, msgOff | null, keyIdx: Uint8Array over n little-endian
  * uint32) -> Uint8Array(n) of statuses   (eddsa.verify against keys of an EdDSA set; h as eddsaVerifyBatch) */
 static napi_value EddsaVerifyBatchKeyed(napi_env env, napi_callback_info info) {
@@ -509,6 +527,7 @@ static napi_value Register(napi_env env, napi_value exports) {
       {"keysetCreate", KeysetCreate}, {"keysetDestroy", KeysetDestroy}, {"ecdsaVerifyBatchKeyed", EcdsaVerifyBatchKeyed},
       {"eddsaKeysetCreate", EddsaKeysetCreate}, {"eddsaVerifyBatchKeyed", EddsaVerifyBatchKeyed},
       {"mulAddBatchKeyed", MulAddBatchKeyed}, {"ecdhDeriveBatchKeyed", EcdhDeriveBatchKeyed},
+      {"ecdsaRecoveryParamBatchKeyed", EcdsaRecoveryParamBatchKeyed},
       {"eddsaSigningSetCreate", EddsaSigningSetCreate}, {"eddsaSignBatchKeyed", EddsaSignBatchKeyed}};
   for (unsigned i = 0; i < sizeof fns / sizeof fns[0]; i++) {
     napi_value f;

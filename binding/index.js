@@ -98,12 +98,13 @@ elliptic.ec.prototype.verifyBatchWire = function verifyBatchWire(hashes, ders, k
 };
 
 // EC#keySet(pubs[, enc]) -> {status, tableBits, deviceBytes, verifyBatch(msgs, sigs, keyIdx[, options]), mul(keyIdx, ks),
-// mulAdd(k1s, keyIdx, k2s), derive(privs, keyIdx), destroy()}: the batch form of `key = ec.keyFromPublic(pub, enc);
-// key.getPublic().precompute()` once and key.verify(msg, sig), pub.mul(k), G.mulAdd(k1, pub, k2) (Arrays of Points) and
-// keyPair.derive(pub) (an Array of BN) many times.  The keys are imported here (a key that throws, throws here, as
-// keyFromPublic does) and kept on the GPU with their tables.  mul and mulAdd take their scalars as Short#mulBatch and
-// Short#mulAddBatch do, and an off-curve key's result is theirs for that point, not the reference's precomputed-point
-// schedule.
+// mulAdd(k1s, keyIdx, k2s), derive(privs, keyIdx), getKeyRecoveryParam(msgs, sigs, keyIdx[, enc]), destroy()}: the batch
+// form of `key = ec.keyFromPublic(pub, enc); key.getPublic().precompute()` once and key.verify(msg, sig), pub.mul(k),
+// G.mulAdd(k1, pub, k2) (Arrays of Points), keyPair.derive(pub) (an Array of BN) and
+// ec.getKeyRecoveryParam(msg, sig, pub) (an Array of numbers, throwing where a loop over that call would) many times.
+// The keys are imported here (a key that throws, throws here, as keyFromPublic does) and kept on the GPU with their
+// tables.  mul and mulAdd take their scalars as Short#mulBatch and Short#mulAddBatch do, and an off-curve key's result
+// is theirs for that point, not the reference's precomputed-point schedule.
 elliptic.ec.prototype.keySet = function keySet(pubs, enc) {
   var id = curveId(this), self = this, len = this.curve.p.byteLength();
   if (id === undefined || this.curve.type !== 'short') throw new Error('key sets: short preset curves only');
@@ -142,6 +143,30 @@ elliptic.ec.prototype.keySet = function keySet(pubs, enc) {
       for (var i = 0; i < privs.length; i++) {
         if (res.status[i] !== 1) throw new Error(THROW[res.status[i]]);
         out.push(new BN(res.out.subarray(len * i, len * i + len)));
+      }
+      return out;
+    },
+    getKeyRecoveryParam: function(msgs, sigs, keyIdx, enc) {
+      var n = msgs.length, idx = new Uint32Array(keyIndices(keyIdx).buffer);
+      var S = sigs.map(function(s) { return new Signature(s, enc); });
+      var one = function(i) { return self.getKeyRecoveryParam(msgs[i], sigs[i], keys[idx[i]].getPublic(), enc); };
+      if (S.some(function(s) { return s.r.byteLength() > len; })) return msgs.map(function(_, i) { return one(i); });
+      var todo = [];
+      S.forEach(function(s, i) { if (s.recoveryParam === null) todo.push(i); });
+      var res = null;
+      if (todo.length) {
+        var e = pack(todo, len, function(i) { return be(new BN(msgs[i]).umod(self.n), len); });
+        var r = pack(todo, len, function(i) { return be(S[i].r, len); });
+        var s = pack(todo, len, function(i) { return be(S[i].s.umod(self.n), len); });
+        var ti = Uint32Array.from(todo, function(i) { return idx[i]; });
+        res = native.ecdsaRecoveryParamBatchKeyed(set.handle, e, r, s, new Uint8Array(ti.buffer));
+      }
+      var out = new Array(n), k = 0;
+      for (var i = 0; i < n; i++) {
+        if (k < todo.length && todo[k] === i) {
+          if (res.status[k] !== 1) throw new Error('Unable to find valid recovery factor');
+          out[i] = res.recid[k++];
+        } else out[i] = one(i);
       }
       return out;
     },

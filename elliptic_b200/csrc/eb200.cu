@@ -2260,6 +2260,51 @@ int mul_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* k1, co
     });
 }
 
+// Keyed getKeyRecoveryParam of one block on one device of the set, chunked like mul_keyed_on.  Launches per chunk: the
+// unkeyed recovery-parameter prep (recovery_param.cu), keyed main, recid normalisation, cold (keyset_recovery_param.cu).
+int recovery_param_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
+                            const u32* key_idx, uint8_t* out_recid, uint8_t* status) {
+  const int curve = ks->curve;
+  const KeysetDev& d = ks->dev[c.device];
+  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
+  int rc = ensure_table(c, curve);
+  if (rc) return rc;
+  const size_t len = curve_len(curve), limbs = (size_t)keyset_geom(curve).limbs;
+  const ChunkPlan P = make_plan(n);
+  const size_t idx_bytes = align256(n * 4);
+  if ((rc = grow(&c.d_in, &c.d_in_cap, idx_bytes + align256(n * 3 * len) + n + 256))) return rc;
+  const WsLayout W = ws_layout(curve, P.max_m);
+  const size_t ws_slot = align256(W.qtab + 2 * limbs * P.max_m * 4);   // prep words | inversion scratch | Y, Z
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, (P.chunks > 1 ? 2 : 1) * ws_slot))) return rc;
+  if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
+  u32* d_idx = (u32*)c.d_in;
+  uint8_t *d_e = c.d_in + idx_bytes, *d_r = d_e + n * len, *d_s = d_r + n * len, *d_id = c.d_in + idx_bytes + align256(n * 3 * len);
+  return run_chunked(c, P,
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {d_e + lo * len, e + lo * len, m * len};
+      seg[1] = {d_r + lo * len, r + lo * len, m * len};
+      seg[2] = {d_s + lo * len, s + lo * len, m * len};
+      seg[3] = {d_idx + lo, key_idx + lo, m * 4};
+      return 4;
+    },
+    [&](size_t lo, size_t m, Launch& L, int slot, int k) {
+      uint8_t* base = c.d_ws + (size_t)slot * ws_slot;
+      u32 *ws = (u32*)(base + W.ws), *scratch = (u32*)(base + W.scratch), *yz = (u32*)(base + W.qtab);
+      cudaError_t err = recovery_param_prep_launch(curve, m, d_e + lo * len, d_r + lo * len, d_s + lo * len, ws, scratch, L.st,
+                                                   &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "recovery_param_prep_launch");
+      const KeyedRecoveryParamArgs a{d_e + lo * len, d_r + lo * len, d_idx + lo, ws, yz, scratch, c.gtab[curve], d_id + lo,
+                                     c.d_status + lo, curve == EB200_CURVE_SECP256K1 ? k256_prep_batch(m) : 0};
+      err = keyset_recovery_param_launch(curve, m, d, a, L.st, c.ev_k0[k], c.ev_k1[k], &L.count);
+      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_recovery_param_launch");
+    },
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {out_recid + lo, d_id + lo, m};
+      seg[1] = {status + lo, c.d_status + lo, m};
+      return 2;
+    });
+}
+
 // ---- EdDSA (ed25519) key sets: kernels in eddsa_keyset.cu, the hash kernel of this file --------------------------------
 // One device's copy: raw keys up, classify + tables, verdicts home.
 int ed_keyset_build_on(Ctx& c, eb200_keyset* ks, const uint8_t* A, uint8_t* key_status) {
@@ -2521,6 +2566,19 @@ int eb200_mul_add_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* k
 int eb200_ecdh_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* priv, const uint32_t* key_idx, uint8_t* out_x,
                                   uint8_t* status) {
   return mul_keyed_common(ks, n, nullptr, priv, key_idx, out_x, status, false, true);
+}
+
+int eb200_ecdsa_recovery_param_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r,
+                                           const uint8_t* s, const uint32_t* key_idx, uint8_t* out_recid, uint8_t* status) {
+  if (!ks || ks->curve == EB200_CURVE_ED25519) return EB200_ERR_ARG;
+  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (n == 0) return EB200_OK;
+  if (!e || !r || !s || !key_idx || !out_recid || !status) return EB200_ERR_ARG;
+  for (size_t i = 0; i < n; i++) if (key_idx[i] >= ks->m) return EB200_ERR_ARG;
+  const size_t len = curve_len(ks->curve);
+  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
+    return recovery_param_keyed_on(c, ks, m, e + lo * len, r + lo * len, s + lo * len, key_idx + lo, out_recid + lo, status + lo);
+  });
 }
 
 int eb200_eddsa_keyset_create(size_t m, const uint8_t* A, uint32_t table_bits, uint8_t* key_status, eb200_keyset** out) {

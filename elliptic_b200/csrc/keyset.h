@@ -1,4 +1,5 @@
-// keyset.h -- the key-set kernels (keyset.cu, keyset_mul.cu, eddsa_keyset.cu, eddsa_signset.cu), launched by eb200.cu
+// keyset.h -- the key-set kernels (keyset.cu, keyset_mul.cu, keyset_recovery_param.cu, eddsa_keyset.cu, eddsa_signset.cu),
+// launched by eb200.cu
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -58,6 +59,26 @@ struct KeyedMulArgs {
 // return cudaErrorInvalidValue.
 cudaError_t keyset_mul_launch(int curve, size_t n, const KeysetDev& k, const KeyedMulArgs& a, cudaStream_t st,
                               cudaEvent_t main_begin, cudaEvent_t main_end, unsigned* launches);
+
+// keyset_recovery_param.cu.  Device buffers of one keyed getKeyRecoveryParam block: e, r (n x len) and key_idx in; ws as
+// the curve's unkeyed recovery-parameter prep left it; yz: 2 x limbs x n words and scratch: limbs x n words of
+// workspace; recid and status (n bytes) out.  batch: items per normalisation thread on secp256k1 (the other curves use
+// SW<C>::BATCH).
+struct KeyedRecoveryParamArgs {
+  const uint8_t *e, *r;
+  const uint32_t* key_idx;
+  const uint32_t* ws;
+  uint32_t *yz, *scratch;
+  const uint32_t* gtab;
+  uint8_t *recid, *status;
+  int batch;
+};
+
+// Launches the keyed main kernel (between main_begin and main_end), the recid normalisation and the cold kernel for
+// s = 0 (mod n) on `st`; adds the kernels launched (three) to *launches.  Other curve ids launch nothing and return
+// cudaErrorInvalidValue.
+cudaError_t keyset_recovery_param_launch(int curve, size_t n, const KeysetDev& k, const KeyedRecoveryParamArgs& a,
+                                         cudaStream_t st, cudaEvent_t main_begin, cudaEvent_t main_end, unsigned* launches);
 
 // ed25519 (eddsa_keyset.cu).  Build: classifies the m raw keys in k.xy and builds their tables on `st`; bases: scratch of
 // m * ed_keyset_windows(W) * 24 words.  Adds the kernels launched (three) to *launches.

@@ -1,6 +1,7 @@
 // recovery_param.cu -- kernels of eb200_ecdsa_recovery_param_batch (EC.getKeyRecoveryParam, ec/index.js:261-278):
 // prep -> main (one u1 G + u2 Q per item: recovery_param_item in ecdsa_k256_body.cuh / ecdsa_sw_body.cuh) -> cold (the
-// s = 0 (mod n) items the main kernel flagged, launched every time like the replay kernels).
+// s = 0 (mod n) items the main kernel flagged, launched every time like the replay kernels).  The keyed call
+// (keyset_recovery_param.cu) runs the same prep through recovery_param_prep_launch.
 //
 // They live in a translation unit of their own.  In eb200.cu's module, even placed after every other kernel, they
 // changed NVVM's inlining into the 255-register p384 / p521 verify, recover and mulAdd kernels (more p521 spills);
@@ -118,6 +119,23 @@ cudaError_t recovery_param_launch(int curve, size_t n, const RecoveryParamArgs& 
     case EB200_CURVE_P521: return sw_launch<P521>(n, a, st, main_begin, main_end, launches);
     case EB200_CURVE_P192: return sw_launch<P192>(n, a, st, main_begin, main_end, launches);
     case EB200_CURVE_P224: return sw_launch<P224>(n, a, st, main_begin, main_end, launches);
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+cudaError_t recovery_param_prep_launch(int curve, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s, u32* ws,
+                                       u32* scratch, cudaStream_t st, unsigned* launches) {
+  const unsigned nb = blocks128(n);
+  switch (curve) {
+    case EB200_CURVE_SECP256K1:
+      RP_LAUNCH((k256_prep_recovery_param_kernel<<<blocks128((n + PREP_BATCH - 1) / PREP_BATCH), 128, 0, st>>>(n, e, r, s, ws,
+                                                                                                               scratch)));
+      return cudaSuccess;
+    case EB200_CURVE_P256: RP_LAUNCH((sw_prep_recovery_param_kernel<P256><<<nb, 128, 0, st>>>(n, e, r, s, ws))); return cudaSuccess;
+    case EB200_CURVE_P384: RP_LAUNCH((sw_prep_recovery_param_kernel<P384><<<nb, 128, 0, st>>>(n, e, r, s, ws))); return cudaSuccess;
+    case EB200_CURVE_P521: RP_LAUNCH((sw_prep_recovery_param_kernel<P521><<<nb, 128, 0, st>>>(n, e, r, s, ws))); return cudaSuccess;
+    case EB200_CURVE_P192: RP_LAUNCH((sw_prep_recovery_param_kernel<P192><<<nb, 128, 0, st>>>(n, e, r, s, ws))); return cudaSuccess;
+    case EB200_CURVE_P224: RP_LAUNCH((sw_prep_recovery_param_kernel<P224><<<nb, 128, 0, st>>>(n, e, r, s, ws))); return cudaSuccess;
     default: return cudaErrorInvalidValue;
   }
 }

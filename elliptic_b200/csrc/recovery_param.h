@@ -17,3 +17,9 @@ struct RecoveryParamArgs {
 // adds the kernels launched to *launches.  Other curve ids launch nothing and return cudaErrorInvalidValue.
 cudaError_t recovery_param_launch(int curve, size_t n, const RecoveryParamArgs& a, cudaStream_t st, cudaEvent_t main_begin,
                                   cudaEvent_t main_end, unsigned* launches);
+
+// The prep kernel alone (u1 = e / s, u2 = (r mod n) / s, FL_INVALID for s = 0 mod n into ws; scratch: the secp256k1
+// inversion's prefix products), for eb200_ecdsa_recovery_param_batch_keyed: its words are laid out as the verify prep's.
+// Adds one launch to *launches.
+cudaError_t recovery_param_prep_launch(int curve, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s, uint32_t* ws,
+                                       uint32_t* scratch, cudaStream_t st, unsigned* launches);

@@ -501,24 +501,7 @@ class EC(_KeyObjects):
         'Unable to find valid recovery factor' (status ST_THROW_NO_RECOVERY)."""
         if self.name not in _SHORT:
             raise EllipticError("get_key_recovery_param_batch: short curves only")
-        n, ln = len(msgs), self._len
-        js = [None] * n
-        st = np.zeros(n, np.uint8)
-        todo = []
-        rss = []
-        for i in range(n):
-            rv, sv = _signature(sigs[i], enc)                  # new Signature(signature, enc) may throw first
-            rp = sigs[i].get("recoveryParam") if isinstance(sigs[i], dict) else \
-                getattr(sigs[i], "recoveryParam", getattr(sigs[i], "recovery_param", None))
-            if rp is not None:
-                js[i], st[i] = rp, nat.ST_TRUE
-                continue
-            if qs[i] is None:
-                raise NeedsReferencePath("Q is the point at infinity")
-            if rv >> (8 * ln):
-                raise NeedsReferencePath("r does not fit the curve's field width")
-            todo.append(i)
-            rss.append((rv, sv))
+        js, st, todo, rss = self._recovery_param_split(msgs, sigs, qs, enc)
         if not todo:
             return js, st
         lib = nat.init(self._device)
@@ -531,6 +514,30 @@ class EC(_KeyObjects):
             st[i] = sub[k]
             js[i] = int(rid[k]) if sub[k] == nat.ST_TRUE else None
         return js, st
+
+    def _recovery_param_split(self, msgs, sigs, qs, enc):
+        """getKeyRecoveryParam's host side before the engine: (js, statuses) with the items whose signature carries a
+        recoveryParam answered (ec/index.js:263-264), and the indices and (r, s) of the others.  qs: the points, or None
+        when a key set supplies them."""
+        n, ln = len(msgs), self._len
+        js = [None] * n
+        st = np.zeros(n, np.uint8)
+        todo = []
+        rss = []
+        for i in range(n):
+            rv, sv = _signature(sigs[i], enc)                  # new Signature(signature, enc) may throw first
+            rp = sigs[i].get("recoveryParam") if isinstance(sigs[i], dict) else \
+                getattr(sigs[i], "recoveryParam", getattr(sigs[i], "recovery_param", None))
+            if rp is not None:
+                js[i], st[i] = rp, nat.ST_TRUE
+                continue
+            if qs is not None and qs[i] is None:
+                raise NeedsReferencePath("Q is the point at infinity")
+            if rv >> (8 * ln):
+                raise NeedsReferencePath("r does not fit the curve's field width")
+            todo.append(i)
+            rss.append((rv, sv))
+        return js, st, todo, rss
 
     def get_key_recovery_param(self, e, signature, Q, enc=None):
         """EC.prototype.getKeyRecoveryParam (ec/index.js:261-278): the parameter, or raises like the reference."""
@@ -799,6 +806,17 @@ class KeySet(_NativeSets):
         self._keyed(nat.load().eb200_ecdh_derive_batch_keyed, (priv,), key_idx, (out, st))
         return out, st
 
+    def recovery_param_batch_packed(self, e, r, s, key_idx):
+        """getKeyRecoveryParam(e, sig, pub) for pub = key key_idx[i] (eb200_ecdsa_recovery_param_batch_keyed): e, r, s are
+        (n, len) uint8 arrays as EC.get_key_recovery_param_batch's call takes them (e, s reduced mod n; r any value below
+        2^(8 len)).  Returns (recid, statuses): recid[i] is the parameter where the status is ST_TRUE, else 0."""
+        key_idx = np.asarray(key_idx)
+        n = len(key_idx)
+        e, r, s = self._packed_scalars("recovery_param_batch_packed", (e, r, s), n)
+        recid, st = np.empty(n, np.uint8), np.empty(n, np.uint8)
+        self._keyed(nat.load().eb200_ecdsa_recovery_param_batch_keyed, (e, r, s), key_idx, (recid, st))
+        return recid, st
+
     def _check_imported(self, key_idx):
         """Raise the reference's error for the first item whose key threw at import, as keyFromPublic would."""
         key_idx = np.asarray(key_idx, np.int64)
@@ -827,6 +845,22 @@ class KeySet(_NativeSets):
         ec = self._ec
         out, st = self.derive_batch_packed(ec._scalars([_bn(p) % ec.n for p in privs]), key_idx)
         return _unpack(out, ec._len, st), st
+
+    def get_key_recovery_param_batch(self, msgs, sigs, key_idx, enc=None):
+        """[ec.getKeyRecoveryParam(msg, sig, pub)] for pub = key key_idx[i]: what EC.get_key_recovery_param_batch returns
+        for those keys' points, (js, statuses), js[i] None where the reference throws 'Unable to find valid recovery
+        factor'.  A signature that carries a recoveryParam is answered with it; a key whose import threw raises its error."""
+        self._check_imported(key_idx)
+        ec = self._ec
+        js, st, todo, rss = ec._recovery_param_split(msgs, sigs, None, enc)
+        if not todo:
+            return js, st
+        recid, sub = self.recovery_param_batch_packed(*ec._recover_args([_msg_int(msgs[i]) for i in todo], rss),
+                                                      np.asarray(key_idx)[todo])
+        for k, i in enumerate(todo):
+            st[i] = sub[k]
+            js[i] = int(recid[k]) if sub[k] == nat.ST_TRUE else None
+        return js, st
 
     def verify_batch(self, msgs, sigs, key_idx, enc=None, msg_bit_length=None):
         """Lists of the reference's message and signature forms, as EC.verify_batch takes them; `enc` is accepted for

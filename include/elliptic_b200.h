@@ -330,6 +330,22 @@ int eb200_mul_add_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* k
 int eb200_ecdh_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* priv, const uint32_t* key_idx, uint8_t* out_x,
                                   uint8_t* status);
 
+/* getKeyRecoveryParam against the keys of a set (`ec.getKeyRecoveryParam(msg, sig, key.getPublic())`, ec/index.js:261-278,
+ * for a signer that does not report the recovery bit): item i uses key key_idx[i].  e, r, s as
+ * eb200_ecdsa_recovery_param_batch takes them (e reduced mod n; r, s any value below 2^(8 len)).  For a key
+ * that imported (key_status TRUE or FALSE), out_recid[i] and status[i] are byte for byte what
+ * eb200_ecdsa_recovery_param_batch writes with q = that key's decoded x || y: an off-curve key gets THROW_NO_RECOVERY (a
+ * recovered point is always on the curve), so no item is replayed.  For a key whose import threw, status[i] is that
+ * throw and out_recid[i] = 0.  u1 G + u2 Q comes from the key's table and the fixed table without doublings, and the
+ * parity of y from one inversion per batch of items.
+ * Argument and lifetime contract as eb200_scalar_mul_batch_keyed: an EdDSA set, a key_idx[i] >= m or a NULL pointer:
+ * EB200_ERR_ARG; a set whose devices eb200_shutdown released: EB200_ERR_NOT_INIT; both before anything is written.
+ * n = 0: EB200_OK.  Host pointers, sharded over the set's devices and chunked with copy / compute overlap.
+ * eb200_last_timing: main_kernel_ms = the keyed main kernel; launches = 4 per chunk (the unkeyed call's scalar prep,
+ * keyed main, recid normalisation, then the cold kernel for s = 0 (mod n)). */
+int eb200_ecdsa_recovery_param_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r,
+                                           const uint8_t* s, const uint32_t* key_idx, uint8_t* out_recid, uint8_t* status);
+
 /* EdDSA key sets: `key = eddsa.keyFromPublic(bytes)` once, then `eddsa.verify(msg, sig, key)` many times
  * (lib/elliptic/eddsa/index.js:52-63, eddsa/key.js:17-44), on ed25519.  The handle is the same eb200_keyset: _info
  * reports EB200_CURVE_ED25519, _destroy and eb200_shutdown treat it as any other set, and passing it to
