@@ -370,6 +370,17 @@ static napi_value EddsaKeysetCreate(napi_env env, napi_callback_info info) {
   int rc = eb200_eddsa_keyset_create(m, A, bits, st, &b->ks);
   return keyset_out(env, rc, b, arr);
 }
+/* x25519KeysetCreate(pubx: m x 32 big-endian, tableBits) -> {handle, status: Uint8Array(m), tableBits, deviceBytes} */
+static napi_value X25519KeysetCreate(napi_env env, napi_callback_info info) {
+  ARGS(2); BUF(0, x, lx); U32(1, bits);
+  size_t m = lx / 32;
+  if (lx % 32) return fail(env, EB200_ERR_ARG);
+  keyset_box* b = (keyset_box*)calloc(1, sizeof *b);
+  if (!b) return fail(env, EB200_ERR_ARG);
+  uint8_t* st; napi_value arr = out_u8(env, m, &st);
+  int rc = eb200_x25519_keyset_create(m, x, bits, st, &b->ks);
+  return keyset_out(env, rc, b, arr);
+}
 /* keysetDestroy(handle): frees the set now; the handle stays valid and answers EB200_ERR_ARG afterwards */
 static napi_value KeysetDestroy(napi_env env, napi_callback_info info) {
   ARGS(1);
@@ -403,7 +414,7 @@ static eb200_keyset* ecdsa_set(napi_env env, napi_value v, size_t* len) {
   int curve = 0;
   if (napi_get_value_external(env, v, &p) != napi_ok || !p || !((keyset_box*)p)->ks) return 0;
   eb200_keyset_info(((keyset_box*)p)->ks, &curve, 0, 0, 0);
-  *len = curve == EB200_CURVE_ED25519 ? 0 : field_len(curve);
+  *len = curve == EB200_CURVE_ED25519 || curve == EB200_CURVE_CURVE25519 ? 0 : field_len(curve);
   return *len ? ((keyset_box*)p)->ks : 0;
 }
 /* mulAddBatchKeyed(handle, k1 | null, k2, keyIdx: Uint8Array over n little-endian uint32) -> {points, status}
@@ -482,6 +493,24 @@ static napi_value EddsaVerifyBatchKeyed(napi_env env, napi_callback_info info) {
   return rc ? fail(env, rc) : arr;
 }
 
+/* x25519DeriveBatchKeyed(handle, priv: n x 32 big-endian (< n), keyIdx: Uint8Array over n little-endian uint32)
+ * -> {out, status}   (KeyPair.derive, ec/key.js:102-107, against key keyIdx[i] of a curve25519 set) */
+static napi_value X25519DeriveBatchKeyed(napi_env env, napi_callback_info info) {
+  ARGS(3); BUF(1, k, lk); BUF(2, idx, li);
+  void* p = 0;
+  if (napi_get_value_external(env, argv[0], &p) != napi_ok || !p || !((keyset_box*)p)->ks) return fail(env, EB200_ERR_ARG);
+  eb200_keyset* ks = ((keyset_box*)p)->ks;
+  size_t n = li / 4;
+  if (li != 4 * n || lk != 32 * n || ((uintptr_t)idx & 3)) return fail(env, EB200_ERR_ARG);
+  uint8_t *out, *st;
+  napi_value ao = out_u8(env, lk, &out), ast = out_u8(env, n, &st);
+  int rc = eb200_x25519_derive_batch_keyed(ks, n, k, (const uint32_t*)(const void*)idx, out, st);
+  if (rc) return fail(env, rc);
+  napi_value res = obj(env);
+  SET(res, "out", ao); SET(res, "status", ast);
+  return res;
+}
+
 /* eddsaSigningSetCreate(secrets: m x 32) -> {handle, pub: Uint8Array(32 m)}   (eddsa.keyFromSecret for m keys) */
 static napi_value EddsaSigningSetCreate(napi_env env, napi_callback_info info) {
   ARGS(1); BUF(0, sec, ls);
@@ -528,7 +557,8 @@ static napi_value Register(napi_env env, napi_value exports) {
       {"eddsaKeysetCreate", EddsaKeysetCreate}, {"eddsaVerifyBatchKeyed", EddsaVerifyBatchKeyed},
       {"mulAddBatchKeyed", MulAddBatchKeyed}, {"ecdhDeriveBatchKeyed", EcdhDeriveBatchKeyed},
       {"ecdsaRecoveryParamBatchKeyed", EcdsaRecoveryParamBatchKeyed},
-      {"eddsaSigningSetCreate", EddsaSigningSetCreate}, {"eddsaSignBatchKeyed", EddsaSignBatchKeyed}};
+      {"eddsaSigningSetCreate", EddsaSigningSetCreate}, {"eddsaSignBatchKeyed", EddsaSignBatchKeyed},
+      {"x25519KeysetCreate", X25519KeysetCreate}, {"x25519DeriveBatchKeyed", X25519DeriveBatchKeyed}};
   for (unsigned i = 0; i < sizeof fns / sizeof fns[0]; i++) {
     napi_value f;
     napi_create_function(env, fns[i].name, NAPI_AUTO_LENGTH, fns[i].cb, 0, &f);

@@ -107,6 +107,7 @@ elliptic.ec.prototype.verifyBatchWire = function verifyBatchWire(hashes, ders, k
 // is theirs for that point, not the reference's precomputed-point schedule.
 elliptic.ec.prototype.keySet = function keySet(pubs, enc) {
   var id = curveId(this), self = this, len = this.curve.p.byteLength();
+  if (id !== undefined && this.curve.type === 'mont') return x25519KeySet(this, pubs, enc);
   if (id === undefined || this.curve.type !== 'short') throw new Error('key sets: short preset curves only');
   init();
   var keys = pubs.map(function(k) { return self.keyFromPublic(k, enc); });
@@ -182,6 +183,35 @@ elliptic.ec.prototype.keySet = function keySet(pubs, enc) {
     return new Uint8Array(idx.buffer);
   }
 };
+
+// EC#keySet(pubs[, enc]) on curve25519 -> {status, tableBits, deviceBytes, derive(privs, keyIdx), destroy()}: the batch
+// form of `pub = ec.keyFromPublic(x, enc)` once and keyPair.derive(pub) (an Array of BN, throwing where a loop over derive
+// would) many times.  A key on the twist imports, as keyFromPublic does (status 5), and its derives throw
+// 'Assertion failed'.  The GPU keeps each key as its edwards25519 image with a per-key table.
+function x25519KeySet(ec, pubs, enc) {
+  init();
+  var keys = pubs.map(function(k) { return ec.keyFromPublic(k, enc); });
+  var set = native.x25519KeysetCreate(pack(keys, 32, function(k) { return be(k.getPublic().getX(), 32); }), 0);
+  return {
+    status: set.status, tableBits: set.tableBits, deviceBytes: set.deviceBytes,
+    derive: function(privs, keyIdx) {
+      if (privs.length !== keyIdx.length) throw new Error('one key index per private key');
+      var idx = new Uint32Array(privs.length), out = [];
+      for (var i = 0; i < privs.length; i++) {
+        if (!(keyIdx[i] >= 0 && keyIdx[i] < keys.length)) throw new Error('key index out of range');
+        idx[i] = keyIdx[i];
+      }
+      var k = pack(privs, 32, function(p) { return be(ec.keyFromPrivate(p).getPrivate(), 32); });
+      var res = native.x25519DeriveBatchKeyed(set.handle, k, new Uint8Array(idx.buffer));
+      for (i = 0; i < privs.length; i++) {
+        if (res.status[i] !== 1) throw new Error(THROW[res.status[i]]);
+        out.push(new BN(res.out.subarray(32 * i, 32 * i + 32)));
+      }
+      return out;
+    },
+    destroy: function() { native.keysetDestroy(set.handle); }
+  };
+}
 
 // EC#signBatch(msgs, keys[, enc][, options]) -> Array<Signature>.  options: canonical, pers / persEnc (one string for the
 // batch), k: function(item, iter) -> BN (the reference's options.k per item), msgBitLength.

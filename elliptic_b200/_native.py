@@ -35,6 +35,7 @@ EXPORTS = [
     "eb200_eddsa_keyset_create", "eb200_eddsa_verify_batch_keyed", "eb200_eddsa_verify_batch_keyed_msgs",
     "eb200_scalar_mul_batch_keyed", "eb200_mul_add_batch_keyed", "eb200_ecdh_derive_batch_keyed",
     "eb200_eddsa_signing_set_create", "eb200_eddsa_sign_batch_keyed", "eb200_ecdsa_recovery_param_batch_keyed",
+    "eb200_x25519_keyset_create", "eb200_x25519_derive_batch_keyed",
 ]
 
 
@@ -113,6 +114,8 @@ def load():
     lib.eb200_eddsa_verify_batch_keyed_msgs.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 6
     lib.eb200_eddsa_signing_set_create.argtypes = [c.c_size_t, c.c_void_p, c.c_void_p, c.POINTER(c.c_void_p)]
     lib.eb200_eddsa_sign_batch_keyed.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 5
+    lib.eb200_x25519_keyset_create.argtypes = [c.c_size_t, c.c_void_p, c.c_uint32, c.c_void_p, c.POINTER(c.c_void_p)]
+    lib.eb200_x25519_derive_batch_keyed.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 4
     lib.eb200_ecdsa_verify_batch_der.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 4 + [c.c_uint32, c.c_void_p]
     lib.eb200_ecdh_derive_batch.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 4
     lib.eb200_scalar_mul_batch.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 4

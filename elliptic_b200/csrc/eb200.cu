@@ -2435,12 +2435,81 @@ int eddsa_sign_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t*
     });
 }
 
+// ---- curve25519 key sets: kernels in x25519_keyset.cu ------------------------------------------------------------------
+// One device's copy: keys up, verdicts, Edwards images and tables, verdicts home.
+int x25519_keyset_build_on(Ctx& c, eb200_keyset* ks, const uint8_t* pubx, uint8_t* key_status) {
+  const size_t m = ks->m;
+  const int W = (int)ks->W;
+  int rc;
+  KeysetDev& d = ks->dev[c.device];
+  d.W = W;
+  CK(cudaMalloc(&d.xy, 32 * m));
+  CK(cudaMalloc(&d.kst, m));
+  CK(cudaMalloc(&d.tab, ed_keyset_key_bytes(W) * m));
+  if ((rc = grow(&c.d_in, &c.d_in_cap, 32 * m))) return rc;
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, m * ed_keyset_windows(W) * 24 * 4))) return rc;
+  uint8_t* dx = c.d_in;
+  return run_single(c, {{dx, pubx, 32 * m}},
+    [&](Launch& L) {
+      cudaError_t err = x25519_keyset_build_launch(m, d, dx, (u32*)c.d_ws, L.st, &L.count);
+      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "x25519_keyset_build_launch");
+    },
+    {{key_status, d.kst, m}}, {}, true);
+}
+
+// Keyed curve25519 derive of one block on one device of the set, chunked like mul_keyed_on.  Launches per chunk: keyed
+// main, normalisation.  The private scalars and the workspace that holds the per-item results are cleared on the
+// chunk's stream behind its kernels.
+int x25519_derive_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* priv, const u32* key_idx, uint8_t* out,
+                           uint8_t* status) {
+  const KeysetDev& d = ks->dev[c.device];
+  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
+  int rc;
+  const ChunkPlan P = make_plan(n);
+  const size_t idx_bytes = align256(n * 4), k_bytes = align256(n * 32);
+  if ((rc = grow(&c.d_in, &c.d_in_cap, idx_bytes + k_bytes + n * 32))) return rc;
+  const size_t ws_slot = align256(x25519_keyset_ws_bytes(P.max_m));
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, (P.chunks > 1 ? 2 : 1) * ws_slot))) return rc;
+  if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
+  u32* d_idx = (u32*)c.d_in;
+  uint8_t *d_k = c.d_in + idx_bytes, *d_out = d_k + k_bytes;
+  return run_chunked(c, P,
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {d_k + 32 * lo, priv + 32 * lo, 32 * m};
+      seg[1] = {d_idx + lo, key_idx + lo, 4 * m};
+      return 2;
+    },
+    [&](size_t lo, size_t m, Launch& L, int slot, int k) {
+      uint8_t* ws = c.d_ws + (size_t)slot * ws_slot;
+      cudaError_t err = x25519_keyset_derive_launch(m, d, d_k + 32 * lo, d_idx + lo, (u32*)ws, d_out + 32 * lo, c.d_status + lo,
+                                                    L.st, c.ev_k0[k], c.ev_k1[k], &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "x25519_keyset_derive_launch");
+      CK(cudaMemsetAsync(d_k + 32 * lo, 0, 32 * m, L.st));              // the private scalars
+      CK(cudaMemsetAsync(ws, 0, x25519_keyset_ws_bytes(m), L.st));      // the per-item results
+      return EB200_OK;
+    },
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {out + 32 * lo, d_out + 32 * lo, 32 * m};
+      seg[1] = {status + lo, c.d_status + lo, m};
+      return 2;
+    });
+}
+
 // h < n for a 32-byte little-endian h (the keyed tables cover 253 bits)
 bool ed_scalar_below_n(const uint8_t* h) {
   static const uint8_t n_le[32] = {0xed, 0xd3, 0xf5, 0x5c, 0x1a, 0x63, 0x12, 0x58, 0xd6, 0x9c, 0xf7, 0xa2, 0xde, 0xf9, 0xde, 0x14,
                                    0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0x10};
   for (int b = 31; b >= 0; b--)
     if (h[b] != n_le[b]) return h[b] < n_le[b];
+  return false;
+}
+// priv < n for a 32-byte big-endian curve25519 private key (the keyed tables cover 253 bits); most keys are decided by
+// their first byte
+bool x25519_priv_below_n(const uint8_t* k) {
+  static const uint8_t n_be[32] = {0x10, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0,
+                                   0x14, 0xde, 0xf9, 0xde, 0xa2, 0xf7, 0x9c, 0xd6, 0x58, 0x12, 0x63, 0x1a, 0x5c, 0xf5, 0xd3, 0xed};
+  for (int b = 0; b < 32; b++)
+    if (k[b] != n_be[b]) return k[b] < n_be[b];
   return false;
 }
 
@@ -2524,7 +2593,7 @@ int eb200_keyset_destroy(eb200_keyset* ks) {
 
 int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r,
                                    const uint8_t* s, const uint32_t* key_idx, uint8_t* status) {
-  if (!ks || ks->curve == EB200_CURVE_ED25519) return EB200_ERR_ARG;      // an EdDSA set: eb200_eddsa_verify_batch_keyed
+  if (!ks || !keyset_geom(ks->curve).limbs) return EB200_ERR_ARG;      // an EdDSA or curve25519 set
   if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
   if (n == 0) return EB200_OK;
   if (!e || !r || !s || !key_idx || !status) return EB200_ERR_ARG;
@@ -2540,7 +2609,7 @@ int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8
 // The three keyed multiplication calls: their argument checks, then the set's devices.
 static int mul_keyed_common(const eb200_keyset* ks, size_t n, const uint8_t* k1, const uint8_t* k2, const uint32_t* key_idx,
                             uint8_t* out, uint8_t* status, bool need_k1, bool derive) {
-  if (!ks || ks->curve == EB200_CURVE_ED25519) return EB200_ERR_ARG;
+  if (!ks || !keyset_geom(ks->curve).limbs) return EB200_ERR_ARG;
   if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
   if (n == 0) return EB200_OK;
   if (!k2 || (need_k1 && !k1) || !key_idx || !out || !status) return EB200_ERR_ARG;
@@ -2570,7 +2639,7 @@ int eb200_ecdh_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_
 
 int eb200_ecdsa_recovery_param_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r,
                                            const uint8_t* s, const uint32_t* key_idx, uint8_t* out_recid, uint8_t* status) {
-  if (!ks || ks->curve == EB200_CURVE_ED25519) return EB200_ERR_ARG;
+  if (!ks || !keyset_geom(ks->curve).limbs) return EB200_ERR_ARG;
   if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
   if (n == 0) return EB200_OK;
   if (!e || !r || !s || !key_idx || !out_recid || !status) return EB200_ERR_ARG;
@@ -2645,6 +2714,32 @@ int eb200_eddsa_sign_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t
   });
   if (rc == EB200_OK) memset(status, EB200_ST_TRUE, n);         // the reference cannot fail here
   return rc;
+}
+
+int eb200_x25519_keyset_create(size_t m, const uint8_t* pubx, uint32_t table_bits, uint8_t* key_status, eb200_keyset** out) {
+  if (out) *out = nullptr;
+  if (!out || !pubx || !key_status || m == 0 || m > 0xffffffffull) return EB200_ERR_ARG;
+  if (table_bits && (table_bits < EB200_KEYSET_MIN_BITS || table_bits > EB200_KEYSET_MAX_BITS)) return EB200_ERR_ARG;
+  if (!table_bits && !(table_bits = ed_keyset_choose_bits(m, EB200_KEYSET_DEFAULT_BUDGET))) {
+    snprintf(g_err, sizeof g_err, "the tables of %zu keys do not fit the default budget at any width: pass table_bits", m);
+    return EB200_ERR_ARG;
+  }
+  eb200_keyset* ks = new eb200_keyset;
+  ks->curve = EB200_CURVE_CURVE25519; ks->m = m; ks->W = table_bits;
+  ks->device_bytes = 32 * m + m + ed_keyset_key_bytes((int)table_bits) * m;
+  return keyset_create_on_devices(ks, out, [&](Ctx& c) { return x25519_keyset_build_on(c, ks, pubx, key_status); });
+}
+
+int eb200_x25519_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* priv, const uint32_t* key_idx,
+                                    uint8_t* out_x, uint8_t* status) {
+  if (!ks || ks->curve != EB200_CURVE_CURVE25519) return EB200_ERR_ARG;
+  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (n == 0) return EB200_OK;
+  if (!priv || !key_idx || !out_x || !status) return EB200_ERR_ARG;
+  for (size_t i = 0; i < n; i++) if (key_idx[i] >= ks->m || !x25519_priv_below_n(priv + 32 * i)) return EB200_ERR_ARG;
+  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
+    return x25519_derive_keyed_on(c, ks, m, priv + 32 * lo, key_idx + lo, out_x + 32 * lo, status + lo);
+  });
 }
 
 }  // extern "C"

@@ -1,5 +1,5 @@
-// keyset.h -- the key-set kernels (keyset.cu, keyset_mul.cu, keyset_recovery_param.cu, eddsa_keyset.cu, eddsa_signset.cu),
-// launched by eb200.cu
+// keyset.h -- the key-set kernels (keyset.cu, keyset_mul.cu, keyset_recovery_param.cu, eddsa_keyset.cu, eddsa_signset.cu,
+// x25519_keyset.cu), launched by eb200.cu
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -12,6 +12,9 @@
 // of each key in `xy`, its verdict (EB200_ST_TRUE or the decoder's throw) in `kst` and ed_keyset_key_bytes() per key.
 // An ed25519 signing set (eddsa_signset.cu) keeps each key's encoded A in `xy` and its secret words in `tab`: a
 // (Montgomery form mod n) then the 32-byte message prefix, ED_SIGNSET_KEY_BYTES per key; `kst` is NULL and W = 0.
+// A curve25519 set (x25519_keyset.cu) keeps in `xy` the ed25519 encoding of each key's Edwards image (zeros for a key
+// that is not TRUE), its verdict (EB200_ST_TRUE or EB200_ST_THROW_ASSERT) in `kst` and the ed25519 set's tables in
+// `tab`, ed_keyset_key_bytes() per key.
 struct KeysetDev {
   uint8_t* xy;
   uint8_t* kst;
@@ -105,3 +108,17 @@ size_t ed_signset_nonce_bytes(size_t n);
 cudaError_t ed_signset_sign_launch(size_t n, const KeysetDev& k, const uint8_t* msgs, const uint64_t* msg_off,
                                    const uint32_t* key_idx, const uint32_t* gtab, uint32_t* ws, uint8_t* sig, cudaStream_t st,
                                    cudaEvent_t main_begin, cudaEvent_t main_end, unsigned* launches);
+
+// curve25519 key sets (x25519_keyset.cu).  Build: classifies the m keys (pubx: m x 32 big-endian, on the device), writes
+// their Edwards images to k.xy and builds their tables on `st`; bases: scratch of m * ed_keyset_windows(W) * 24 words.
+// Adds the kernels launched (three) to *launches.
+cudaError_t x25519_keyset_build_launch(size_t m, const KeysetDev& k, const uint8_t* pubx, uint32_t* bases, cudaStream_t st,
+                                       unsigned* launches);
+// Workspace of a derive launch of n items.
+size_t x25519_keyset_ws_bytes(size_t n);
+// Derive: priv (n x 32 big-endian, each < n) and key_idx in, out (n x 32 big-endian u) and status out; ws:
+// x25519_keyset_ws_bytes(n).  Launches the keyed main kernel (between main_begin and main_end) and the normalisation on
+// `st` and adds two to *launches.
+cudaError_t x25519_keyset_derive_launch(size_t n, const KeysetDev& k, const uint8_t* priv, const uint32_t* key_idx, uint32_t* ws,
+                                        uint8_t* out, uint8_t* status, cudaStream_t st, cudaEvent_t main_begin,
+                                        cudaEvent_t main_end, unsigned* launches);

@@ -256,7 +256,10 @@ class _KeyObjects:
     """The key-object side of the `ec` API (ec/key.js), in batch form; EC inherits it."""
 
     def key_set(self, keys, enc=None, table_bits=0):
-        """The batch form of `key = ec.keyFromPublic(pub, enc)` + `key.getPublic().precompute()`: a KeySet on the GPU."""
+        """The batch form of `key = ec.keyFromPublic(pub, enc)` + `key.getPublic().precompute()`: a KeySet on the GPU
+        (an X25519KeySet on curve25519)."""
+        if self.name == "curve25519":
+            return X25519KeySet(self, keys, table_bits)
         return KeySet(self, keys, enc, table_bits)
 
 
@@ -882,3 +885,57 @@ class KeySet(_NativeSets):
             if st[i] in (nat.ST_TRUE, nat.ST_FALSE, nat.ST_NEEDS_HOST):
                 st[i] = v
         return st
+
+
+class X25519KeySet(_NativeSets):
+    """curve25519 peer keys imported once (eb200_x25519_keyset_create) and kept on the GPU as their edwards25519 images
+    with per-key tables; item i of a derive call uses key key_idx[i].  Keys come in the forms EC.derive_batch takes on
+    curve25519 (int, hex or big-endian bytes, reduced mod p when wider than 256 bits).  `status`: per key, ST_TRUE, or
+    ST_THROW_ASSERT for a point on the twist (whose derives then give that status, as in EC.derive_batch).  close()
+    frees the device memory; the object is a context manager."""
+
+    def __init__(self, ec, keys, table_bits=0):
+        self._ec = ec
+        p = ec._c["p"]
+        pubx = _pack((x % p if x >> 256 else x for x in (_bn(k) for k in keys)), 32)
+        lib = nat.init(ec._device)
+        self.status = np.zeros(len(pubx), np.uint8)
+        h = ctypes.c_void_p()
+        nat.check(lib.eb200_x25519_keyset_create(len(pubx), pubx.ctypes.data, table_bits, self.status.ctypes.data,
+                                                 ctypes.byref(h)))
+        self._sets = [h]
+        w, db = ctypes.c_uint32(), ctypes.c_size_t()
+        nat.check(lib.eb200_keyset_info(h, None, None, ctypes.byref(w), ctypes.byref(db)))
+        self.table_bits, self.device_bytes = w.value, db.value
+
+    def derive_batch_packed(self, priv, key_idx, out=None, status=None):
+        """keyPair.derive(pub) for pub = key key_idx[i] (eb200_x25519_derive_batch_keyed): priv is an (n, 32) uint8 array,
+        big-endian, each below n (reduced mod n as _importPrivate does, ec/key.js:76-82).  Returns ((n, 32) shared x
+        big-endian, statuses), as EC.derive_batch_packed for those keys; `out` / `status` let the caller supply (and
+        reuse) the result buffers, e.g. pinned ones."""
+        priv = np.ascontiguousarray(priv, dtype=np.uint8)
+        key_idx = np.asarray(key_idx)
+        n = len(key_idx)
+        if priv.shape != (n, 32) or key_idx.shape != (n,):
+            raise ValueError("derive_batch_packed: priv must be an (n, 32) uint8 array, n = len(key_idx)")
+        if n and (key_idx.min() < 0 or key_idx.max() >= len(self.status)):
+            raise ValueError("key_idx out of range")
+        out = np.empty((n, 32), np.uint8) if out is None else out
+        st = np.empty(n, np.uint8) if status is None else status
+        if out.shape != (n, 32) or out.dtype != np.uint8 or not out.flags.c_contiguous or st.shape != (n,) or st.dtype != np.uint8:
+            raise ValueError("derive_batch_packed: out must be a contiguous (n, 32) uint8 array, status (n,) uint8")
+        if not self._sets:
+            if n:
+                raise EllipticError("key set is closed")
+            return out, st
+        nat.call(nat.load().eb200_x25519_derive_batch_keyed, self._sets[0], n, priv, np.ascontiguousarray(key_idx, np.uint32),
+                 out, st)
+        return out, st
+
+    def derive_batch(self, privs, key_idx):
+        """[keyPair(priv).derive(pub)] for pub = key key_idx[i]: what EC.derive_batch returns for those keys, (values,
+        statuses); a twist key's items are None with ST_THROW_ASSERT."""
+        if len(privs) != len(key_idx):
+            raise ValueError("derive_batch: one key index per private key")
+        out, st = self.derive_batch_packed(_pack((_bn(k) % self._ec.n for k in privs), 32), key_idx)
+        return _unpack(out, 32, st), st

@@ -266,8 +266,9 @@ int eb200_eddsa_sign_batch(size_t n, const uint8_t* secrets, const uint8_t* msgs
 /* Key sets: the batch form of the reference's key objects -- `key = ec.keyFromPublic(pub, enc)` once,
  * `key.getPublic().precompute()` (lib/elliptic/curve/base.js:312-327), then `key.verify(msg, sig)` many times
  * (lib/elliptic/ec/key.js:20-28, 84-99, 114-116).  A set holds m public keys of one short preset (secp256k1, p256, p384,
- * p521, p192, p224; the 25519 curves return EB200_ERR_UNSUPPORTED here, and ed25519 EdDSA keys have
- * eb200_eddsa_keyset_create below) on the GPU: decoded once, checked against the curve
+ * p521, p192, p224; the 25519 curves return EB200_ERR_UNSUPPORTED here: ed25519 EdDSA keys have
+ * eb200_eddsa_keyset_create and curve25519 ECDH keys eb200_x25519_keyset_create below) on the GPU: decoded once, checked
+ * against the curve
  * once, and each on-curve key with a table of its multiples (2i+1) 2^(W j) Q over W-bit windows, so that a keyed verify
  * needs no doubling and no per-item table.
  *   pub, pub_fmt : m keys, exactly what eb200_ecdsa_verify_batch takes
@@ -317,9 +318,9 @@ int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8
  * replay the unkeyed call's schedule for an arbitrary point on the key's coordinates, derive is THROW_NOT_VALIDATED.
  * That is not the reference's _fixedNafMul schedule for a precomputed point, whose answer for an off-curve point
  * differs; eb200_ecdsa_verify_batch_keyed follows the same convention.
- * An EdDSA set, a key_idx[i] >= m or a NULL pointer: EB200_ERR_ARG; a set whose devices eb200_shutdown released:
- * EB200_ERR_NOT_INIT; both before anything is written.  n = 0: EB200_OK.  Host pointers, sharded over the set's devices
- * and chunked with copy / compute overlap as eb200_ecdsa_verify_batch_keyed.  derive clears the private scalars, their
+ * An EdDSA or curve25519 set, a key_idx[i] >= m or a NULL pointer: EB200_ERR_ARG; a set whose devices eb200_shutdown
+ * released: EB200_ERR_NOT_INIT; both before anything is written.  n = 0: EB200_OK.  Host pointers, sharded over the set's
+ * devices and chunked with copy / compute overlap as eb200_ecdsa_verify_batch_keyed.  derive clears the private scalars, their
  * digit words and the Jacobian results from the library's device buffers before it returns.
  * eb200_last_timing: main_kernel_ms = the keyed main kernel; launches = 4 per chunk (scalar prep, keyed main, batched
  * normalisation to affine, then the keyed replay of off-curve-key items, or for derive the status map). */
@@ -338,7 +339,8 @@ int eb200_ecdh_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_
  * recovered point is always on the curve), so no item is replayed.  For a key whose import threw, status[i] is that
  * throw and out_recid[i] = 0.  u1 G + u2 Q comes from the key's table and the fixed table without doublings, and the
  * parity of y from one inversion per batch of items.
- * Argument and lifetime contract as eb200_scalar_mul_batch_keyed: an EdDSA set, a key_idx[i] >= m or a NULL pointer:
+ * Argument and lifetime contract as eb200_scalar_mul_batch_keyed: an EdDSA or curve25519 set, a key_idx[i] >= m or a
+ * NULL pointer:
  * EB200_ERR_ARG; a set whose devices eb200_shutdown released: EB200_ERR_NOT_INIT; both before anything is written.
  * n = 0: EB200_OK.  Host pointers, sharded over the set's devices and chunked with copy / compute overlap.
  * eb200_last_timing: main_kernel_ms = the keyed main kernel; launches = 4 per chunk (the unkeyed call's scalar prep,
@@ -398,6 +400,36 @@ int eb200_eddsa_signing_set_create(size_t m, const uint8_t* secrets, uint8_t* ou
  * returns.  eb200_last_timing: main_kernel_ms = the nonce kernel; launches = 3 per chunk. */
 int eb200_eddsa_sign_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* msgs, const uint64_t* msg_off,
                                  const uint32_t* key_idx, uint8_t* out_sig, uint8_t* status);
+
+/* curve25519 key sets: `pub = ec.keyFromPublic(x)` once, then `keyPair.derive(pub)` many times (lib/elliptic/ec/key.js:
+ * 102-107), on curve25519.  The handle is the same eb200_keyset: _info reports EB200_CURVE_CURVE25519, _destroy and
+ * eb200_shutdown treat it as any other set, and passing it to any short-curve or EdDSA keyed call (or any other set to
+ * eb200_x25519_derive_batch_keyed) returns EB200_ERR_ARG.  Each key is kept as its image on edwards25519,
+ * y = (u - 1) / (u + 1), a group isomorphism, with the table of an EdDSA key set: a derive is about 37 table additions
+ * at W = 7 and no doubling, instead of the 256-step ladder.
+ *   pubx       : m x 32 bytes big-endian, as eb200_x25519_derive_batch takes them (any value below 2^256, read mod p)
+ *   table_bits : W as eb200_eddsa_keyset_create (same geometry: ceil(253 / W) windows of 2^(W-1) entries of 96 bytes;
+ *                0 = the widest whose tables fit EB200_KEYSET_DEFAULT_BUDGET bytes per device)
+ *   key_status : m bytes out -- EB200_ST_TRUE if u^3 + 486662 u^2 + u is 0 or a square mod p (MontCurve.validate,
+ *                mont.js:21-28, the unkeyed call's check), else EB200_ST_THROW_ASSERT (a point on the twist)
+ * m = 0, m >= 2^32 or a NULL pointer: EB200_ERR_ARG; no device: EB200_ERR_NOT_INIT; a failed allocation: EB200_ERR_CUDA
+ * with *out NULL and everything freed.  device_bytes = 32 m + m + the tables.  eb200_last_timing after create: the
+ * build kernels of the slowest device; launches = 3 per device (classify, window bases, table windows). */
+int eb200_x25519_keyset_create(size_t m, const uint8_t* pubx, uint32_t table_bits, uint8_t* key_status, eb200_keyset** out);
+/* Batch of keyPair(priv).derive(pub): item i uses key key_idx[i].  priv: n x 32 bytes big-endian, each below n (reduced
+ * mod n at import, as eb200_x25519_derive_batch expects them; the tables cover 253 bits).  out_x and status[i] are byte
+ * for byte what eb200_x25519_derive_batch writes for the same priv with pubx = that key's bytes: TRUE and x(priv P),
+ * 0 for the point at infinity; THROW_ASSERT and 32 zero bytes for a key on the twist.
+ * A NULL pointer, a key_idx[i] >= m or a priv[i] >= n: EB200_ERR_ARG; a set whose devices eb200_shutdown released:
+ * EB200_ERR_NOT_INIT; both before anything is written.  n = 0: EB200_OK.  Host pointers, sharded over the set's
+ * devices and chunked with copy / compute overlap.  Per chunk: the keyed main kernel (one table gather and one
+ * addition per window of priv) and a normalisation (one inversion per 16 items).  The main kernel's table gathers are
+ * indexed by the digits of the private scalar, as in the keyed short-curve derive and the fixed-base signing paths
+ * (the unkeyed ladder's memory accesses do not depend on it).  The staged private scalars and the workspace that holds
+ * the per-item results are cleared from the library's device buffers before the call returns.
+ * eb200_last_timing: main_kernel_ms = the keyed main kernel; launches = 2 per chunk. */
+int eb200_x25519_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* priv, const uint32_t* key_idx,
+                                    uint8_t* out_x, uint8_t* status);
 
 /* Self-test hooks used by the parity tests (device arithmetic vs the oracle).
  * a, b, out: n elements of L little-endian 32-bit limbs each (host pointers); L = 8, except p192 6, p384 12 and
