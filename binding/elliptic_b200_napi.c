@@ -408,6 +408,26 @@ static napi_value EcdsaVerifyBatchKeyed(napi_env env, napi_callback_info info) {
   return rc ? fail(env, rc) : arr;
 }
 
+/* ecdsaVerifyBatchKeyedDer(handle, e, sigs, sigOff (n + 1 little-endian u64 offsets, as a Uint8Array view),
+ * keyIdx: Uint8Array over n little-endian uint32) -> Uint8Array(n) of statuses (DER parsed on the GPU) */
+static napi_value EcdsaVerifyBatchKeyedDer(napi_env env, napi_callback_info info) {
+  ARGS(5); BUF(1, e, le); BUF(2, sig, lsg); BUF(3, off, lo); BUF(4, idx, li);
+  void* p = 0;
+  if (napi_get_value_external(env, argv[0], &p) != napi_ok || !p || !((keyset_box*)p)->ks) return fail(env, EB200_ERR_ARG);
+  eb200_keyset* ks = ((keyset_box*)p)->ks;
+  int curve = 0;
+  eb200_keyset_info(ks, &curve, 0, 0, 0);
+  size_t len = field_len(curve), n = li / 4;
+  if (!len || li != 4 * n || le != n * len || lo != 8 * (n + 1) || ((uintptr_t)off & 7) || ((uintptr_t)idx & 3))
+    return fail(env, EB200_ERR_ARG);
+  const uint64_t* o = (const uint64_t*)(const void*)off;
+  for (size_t i = 0; i < n; i++) if (o[i + 1] < o[i]) return fail(env, EB200_ERR_ARG);
+  if (o[n] > lsg) return fail(env, EB200_ERR_ARG);
+  uint8_t* st; napi_value arr = out_u8(env, n, &st);
+  int rc = eb200_ecdsa_verify_batch_keyed_der(ks, n, e, sig, o, (const uint32_t*)(const void*)idx, st);
+  return rc ? fail(env, rc) : arr;
+}
+
 /* the ECDSA set behind a handle and its field length, or 0 */
 static eb200_keyset* ecdsa_set(napi_env env, napi_value v, size_t* len) {
   void* p = 0;
@@ -554,6 +574,7 @@ static napi_value Register(napi_env env, napi_value exports) {
       {"curveOpBatch", CurveOpBatch}, {"eddsaVerifyBatch", EddsaVerifyBatch}, {"eddsaSignBatch", EddsaSignBatch},
       {"x25519Batch", X25519Batch},
       {"keysetCreate", KeysetCreate}, {"keysetDestroy", KeysetDestroy}, {"ecdsaVerifyBatchKeyed", EcdsaVerifyBatchKeyed},
+      {"ecdsaVerifyBatchKeyedDer", EcdsaVerifyBatchKeyedDer},
       {"eddsaKeysetCreate", EddsaKeysetCreate}, {"eddsaVerifyBatchKeyed", EddsaVerifyBatchKeyed},
       {"mulAddBatchKeyed", MulAddBatchKeyed}, {"ecdhDeriveBatchKeyed", EcdhDeriveBatchKeyed},
       {"ecdsaRecoveryParamBatchKeyed", EcdsaRecoveryParamBatchKeyed},

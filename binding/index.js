@@ -97,11 +97,13 @@ elliptic.ec.prototype.verifyBatchWire = function verifyBatchWire(hashes, ders, k
   return Array.prototype.map.call(st, function(v, i) { return v === 4 ? self.verify(hashes[i], ders[i], keys[i]) : statusToBool(v); });
 };
 
-// EC#keySet(pubs[, enc]) -> {status, tableBits, deviceBytes, verifyBatch(msgs, sigs, keyIdx[, options]), mul(keyIdx, ks),
+// EC#keySet(pubs[, enc]) -> {status, tableBits, deviceBytes, verifyBatch(msgs, sigs, keyIdx[, options]),
+// verifyBatchWire(hashes, ders, keyIdx), mul(keyIdx, ks),
 // mulAdd(k1s, keyIdx, k2s), derive(privs, keyIdx), getKeyRecoveryParam(msgs, sigs, keyIdx[, enc]), destroy()}: the batch
 // form of `key = ec.keyFromPublic(pub, enc); key.getPublic().precompute()` once and key.verify(msg, sig), pub.mul(k),
 // G.mulAdd(k1, pub, k2) (Arrays of Points), keyPair.derive(pub) (an Array of BN) and
 // ec.getKeyRecoveryParam(msg, sig, pub) (an Array of numbers, throwing where a loop over that call would) many times.
+// verifyBatchWire is the keyed EC#verifyBatchWire: hashes of the field length and DER signatures, parsed on the GPU.
 // The keys are imported here (a key that throws, throws here, as keyFromPublic does) and kept on the GPU with their
 // tables.  mul and mulAdd take their scalars as Short#mulBatch and Short#mulAddBatch do, and an off-curve key's result
 // is theirs for that point, not the reference's precomputed-point schedule.
@@ -129,6 +131,12 @@ elliptic.ec.prototype.keySet = function keySet(pubs, enc) {
       }
       var st = native.ecdsaVerifyBatchKeyed(set.handle, e, r, s, new Uint8Array(idx.buffer));
       return Array.prototype.map.call(st, function(v, i) { return i in early ? false : statusToBool(v); });
+    },
+    verifyBatchWire: function(hashes, ders, keyIdx) {
+      if (hashes.some(function(h) { return h.length !== len; })) throw new Error('verifyBatchWire: hashes of ' + len + ' bytes');
+      var idx = keyIndices(keyIdx), sg = concatMsgs(ders);
+      var st = native.ecdsaVerifyBatchKeyedDer(set.handle, pack(hashes, len, function(h) { return h; }), sg.blob, sg.off, idx);
+      return Array.prototype.map.call(st, function(v) { return statusToBool(v); });
     },
     mul: function(keyIdx, ks) {
       var big = new BN(1).ushln(8 * len);          // Short#mulBatch's rule: only a k of 2^(8 len) or more is reduced mod n

@@ -2193,6 +2193,92 @@ int verify_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, 
     });
 }
 
+// The unchanged prep kernel of the set's curve on L's stream (ws / scratch as ws_layout places them), and the curve's
+// replay table for keyset_verify_launch.
+int keyed_verify_prep(Ctx& c, int curve, size_t m, const uint8_t* d_e, const uint8_t* d_r, const uint8_t* d_s, u32* ws,
+                      u32* scratch, Launch& L, const u32** replay) {
+  return with_curve(curve, [&](auto cv) {
+    typedef decltype(cv) T;
+    if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;
+    else if constexpr (is_k256<T>) {
+      L(k256_prep_kernel, batch_blocks(m, k256_prep_batch(m)), 128, m, d_e, d_r, d_s, ws, scratch, k256_prep_batch(m));
+      *replay = c.replay_tab;
+    } else {
+      typedef typename T::C C;
+      L(sw_prep_kernel<C>, batch_blocks(m, SW<C>::BATCH), 128, m, d_e, d_r, d_s, ws, scratch);
+      *replay = c.sw_replay_tab[curve];
+    }
+    return L.rc;
+  });
+}
+
+// Keyed verify of DER signatures, one block on one device of the set, chunked like verify_keyed_on; the variable-length
+// segments as eddsa_sign_keyed_on stages them (sig_off points at this block's first offset, offsets absolute).
+// Launches per chunk: keyed DER decode, prep, keyed main, keyed replay, verdict merge.
+int verify_keyed_der_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* sigs, const uint64_t* sig_off,
+                        const u32* key_idx, uint8_t* status) {
+  const int curve = ks->curve;
+  const KeysetDev& d = ks->dev[c.device];
+  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
+  int rc = ensure_table(c, curve);
+  if (rc) return rc;
+  const size_t len = curve_len(curve);
+  const ChunkPlan P = make_plan(n);
+  const size_t sig_bytes = (size_t)(sig_off[n] - sig_off[0]);
+  const size_t off_bytes = align256((n + 1) * 8);
+  const size_t base = align256(n * 4) + align256(n * 3 * len) + align256(n);   // key_idx | e, r, s | verdicts
+  if ((rc = grow(&c.d_in, &c.d_in_cap, base + off_bytes + align256(sig_bytes + 1)))) return rc;
+  const WsLayout W = ws_layout(curve, P.max_m);
+  const size_t ws_slot = W.qtab;                    // prep words and the inversion scratch; no per-item table
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, (P.chunks > 1 ? 2 : 1) * ws_slot))) return rc;
+  if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
+  u32* d_idx = (u32*)c.d_in;
+  uint8_t *d_e = c.d_in + align256(n * 4), *d_r = d_e + n * len, *d_s = d_r + n * len;
+  uint8_t* d_vd = d_e + align256(n * 3 * len);
+  unsigned long long* d_off = (unsigned long long*)(c.d_in + base);
+  uint8_t* d_sig = c.d_in + base + off_bytes;
+  return run_chunked(c, P,
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {d_e + lo * len, e + lo * len, m * len};
+      seg[1] = {d_idx + lo, key_idx + lo, m * 4};
+      seg[2] = {d_off + lo, sig_off + lo, (m + 1) * 8};
+      seg[3] = {d_sig + (sig_off[lo] - sig_off[0]), sigs + sig_off[lo], (size_t)(sig_off[lo + m] - sig_off[lo])};
+      return 4;
+    },
+    [&](size_t lo, size_t m, Launch& L, int slot, int k) {
+      u32* ws = (u32*)(c.d_ws + (size_t)slot * ws_slot + W.ws);
+      u32* scratch = (u32*)(c.d_ws + (size_t)slot * ws_slot + W.scratch);
+      cudaError_t err = keyset_der_decode_launch(m, (u32)len, d_sig - sig_off[0], d_off + lo, d_idx + lo, d, d_r + lo * len,
+                                                 d_s + lo * len, d_vd + lo, L.st, &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "keyset_der_decode_launch");
+      const u32* replay = nullptr;
+      int rc2 = keyed_verify_prep(c, curve, m, d_e + lo * len, d_r + lo * len, d_s + lo * len, ws, scratch, L, &replay);
+      if (rc2) return rc2;
+      const KeyedVerifyArgs a{d_e + lo * len, d_r + lo * len, d_s + lo * len, d_idx + lo, c.d_status + lo, ws, c.gtab[curve], replay};
+      if ((err = keyset_verify_launch(curve, m, d, a, L.st, c.ev_k0[k], c.ev_k1[k], &L.count)) != cudaSuccess)
+        return cuda_fail(err, "keyset_verify_launch");
+      if ((err = keyset_verdict_merge_launch(m, d_vd + lo, c.d_status + lo, L.st, &L.count)) != cudaSuccess)
+        return cuda_fail(err, "keyset_verdict_merge_launch");
+      return EB200_OK;
+    },
+    [&](size_t lo, size_t m, Seg* seg) {
+      seg[0] = {status + lo, c.d_status + lo, m};
+      return 1;
+    });
+}
+
+// workspace of eb200_ecdsa_verify_batch_keyed_dev: [screened key_idx (n words) | verdicts (n bytes) | prep words and the
+// inversion scratch, as ws_layout places them]
+struct KeyedDevWs { size_t idx, verdict, prep, total; };
+KeyedDevWs keyed_dev_ws(int curve, size_t n) {
+  KeyedDevWs L;
+  L.idx = 0;
+  L.verdict = align256(n * 4);
+  L.prep = L.verdict + align256(n);
+  L.total = L.prep + ws_layout(curve, n).qtab;
+  return L;
+}
+
 // Keyed Point.mul / G.mulAdd / KeyPair.derive of one block on one device of the set, chunked like verify_keyed_on.
 // k1 == NULL: k2 times the key (derive: x only, and an off-curve key is THROW_NOT_VALIDATED instead of replayed);
 // else k1 G + k2 times the key.  Launches per chunk: prep_scalars, keyed main, normalisation, then the keyed replay
@@ -2601,6 +2687,58 @@ int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8
   const size_t len = curve_len(ks->curve);
   return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
     return verify_keyed_on(c, ks, m, e + lo * len, r + lo * len, s + lo * len, key_idx + lo, status + lo);
+  });
+}
+
+int eb200_ecdsa_verify_batch_keyed_der(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* sigs,
+                                       const uint64_t* sig_off, const uint32_t* key_idx, uint8_t* status) {
+  if (!ks || !keyset_geom(ks->curve).limbs) return EB200_ERR_ARG;      // an EdDSA, signing or curve25519 set
+  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (n == 0) return EB200_OK;
+  if (!e || !sigs || !sig_off || !key_idx || !status) return EB200_ERR_ARG;
+  for (size_t i = 0; i < n; i++) if (sig_off[i + 1] < sig_off[i] || key_idx[i] >= ks->m) return EB200_ERR_ARG;
+  const size_t len = curve_len(ks->curve);
+  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
+    return verify_keyed_der_on(c, ks, m, e + lo * len, sigs, sig_off + lo, key_idx + lo, status + lo);
+  });
+}
+
+size_t eb200_ecdsa_verify_keyed_workspace_bytes(const eb200_keyset* ks, size_t n) {
+  if (!ks || !keyset_geom(ks->curve).limbs) return 0;
+  return keyed_dev_ws(ks->curve, n).total;
+}
+
+int eb200_ecdsa_verify_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_e, const uint8_t* d_r,
+                                       const uint8_t* d_s, const uint32_t* d_key_idx, uint8_t* d_status,
+                                       void* d_workspace, void* stream) {
+  if (!ks || !keyset_geom(ks->curve).limbs) return EB200_ERR_ARG;
+  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (n == 0) return EB200_OK;
+  if (!d_e || !d_r || !d_s || !d_key_idx || !d_status || !d_workspace) return EB200_ERR_ARG;
+  const Ctx* owner = ctx_of(d_status);
+  if (!owner) return EB200_ERR_NOT_INIT;
+  const KeysetDev& d = ks->dev[owner->device];
+  if (!d.tab) return EB200_ERR_ARG;                // an initialised device that does not hold this set
+  const int curve = ks->curve;
+  return run_dev(d_status, curve, stream, [&](Ctx& c, Launch& L) {
+    const KeyedDevWs Lw = keyed_dev_ws(curve, n);
+    const WsLayout W = ws_layout(curve, n);
+    uint8_t* base = (uint8_t*)d_workspace;
+    u32* idx = (u32*)(base + Lw.idx);
+    uint8_t* vd = base + Lw.verdict;
+    u32* ws = (u32*)(base + Lw.prep + W.ws);
+    u32* scratch = (u32*)(base + Lw.prep + W.scratch);
+    cudaError_t err = keyset_index_screen_launch(n, d_key_idx, ks->m, idx, vd, L.st, &L.count);
+    if (err != cudaSuccess) return cuda_fail(err, "keyset_index_screen_launch");
+    const u32* replay = nullptr;
+    int rc = keyed_verify_prep(c, curve, n, d_e, d_r, d_s, ws, scratch, L, &replay);
+    if (rc) return rc;
+    const KeyedVerifyArgs a{d_e, d_r, d_s, idx, d_status, ws, c.gtab[curve], replay};
+    if ((err = keyset_verify_launch(curve, n, d, a, L.st, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END], &L.count)) != cudaSuccess)
+      return cuda_fail(err, "keyset_verify_launch");
+    if ((err = keyset_verdict_merge_launch(n, vd, d_status, L.st, &L.count)) != cudaSuccess)
+      return cuda_fail(err, "keyset_verdict_merge_launch");
+    return EB200_OK;
   });
 }
 

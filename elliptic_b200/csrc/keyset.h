@@ -1,5 +1,5 @@
-// keyset.h -- the key-set kernels (keyset.cu, keyset_mul.cu, keyset_recovery_param.cu, eddsa_keyset.cu, eddsa_signset.cu,
-// x25519_keyset.cu), launched by eb200.cu
+// keyset.h -- the key-set kernels (keyset.cu, keyset_forms.cu, keyset_mul.cu, keyset_recovery_param.cu, eddsa_keyset.cu,
+// eddsa_signset.cu, x25519_keyset.cu), launched by eb200.cu
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -40,6 +40,21 @@ struct KeyedVerifyArgs {
 // adds the kernels launched (two) to *launches.  Other curve ids launch nothing and return cudaErrorInvalidValue.
 cudaError_t keyset_verify_launch(int curve, size_t n, const KeysetDev& k, const KeyedVerifyArgs& a, cudaStream_t st,
                                  cudaEvent_t main_begin, cudaEvent_t main_end, unsigned* launches);
+
+// keyset_forms.cu: the kernels around keyset_verify_launch for the DER and device-pointer forms of the keyed verify.  Each
+// launches one kernel on `st` and adds it to *launches.  verdict: n bytes, 0 = the keyed status stands, else the item's
+// status (keyset_forms_body.cuh).
+// DER decode: der / off as der_decode_kernel takes them (n + 1 offsets into der); writes r, s (n x len; zeros for a
+// rejected encoding) for the unchanged prep kernel, and per item the key's import throw (k.kst[key_idx[i]]), else
+// EB200_ST_THROW_SIG_FORMAT for a rejected encoding, else 0.
+cudaError_t keyset_der_decode_launch(size_t n, uint32_t len, const uint8_t* der, const unsigned long long* off,
+                                     const uint32_t* key_idx, const KeysetDev& k, uint8_t* r, uint8_t* s, uint8_t* verdict,
+                                     cudaStream_t st, unsigned* launches);
+// Index screen: idx_out[i] = key_idx[i] when it is below m, else 0 with verdict EB200_ST_BAD_KEY_INDEX.
+cudaError_t keyset_index_screen_launch(size_t n, const uint32_t* key_idx, size_t m, uint32_t* idx_out, uint8_t* verdict,
+                                       cudaStream_t st, unsigned* launches);
+// Verdict merge, behind the keyed replay: status[i] = verdict[i] wherever that is not 0.
+cudaError_t keyset_verdict_merge_launch(size_t n, const uint8_t* verdict, uint8_t* status, cudaStream_t st, unsigned* launches);
 
 // keyset_mul.cu.  Device buffers of one keyed mul / mulAdd / derive block: k1 (NULL: no base-point term), k2 (n x len, as the caller
 // gave them: the replay uses them unreduced) and key_idx in; ws as the curve's unkeyed prep_scalars kernel left it;

@@ -780,6 +780,37 @@ class KeySet(_NativeSets):
         self._keyed(lib.eb200_ecdsa_verify_batch_keyed, (e, r, s), key_idx, (status,))
         return status
 
+    def verify_batch_der_packed(self, e, ders, key_idx):
+        """e: (n, len) uint8 truncated hashes; ders: n DER byte strings, parsed on the GPU exactly as
+        EC.verify_batch_der_packed parses them; key_idx: n indices into the set.  Returns the status bytes
+        EC.verify_batch_der_packed gives with pub[i] = key key_idx[i] (eb200_ecdsa_verify_batch_keyed_der)."""
+        lib = nat.load()
+        ln = self._ec._len
+        ders = [bytes(d) for d in ders]
+        e = np.ascontiguousarray(e, dtype=np.uint8)
+        key_idx = np.asarray(key_idx)
+        n = len(ders)
+        if not (e.shape == (n, ln) and key_idx.shape == (n,)):
+            raise ValueError("e must be (n, %d) uint8, ders n byte strings and key_idx (n,)" % ln)
+        if n and (key_idx.min() < 0 or key_idx.max() >= len(self.status)):
+            raise ValueError("key_idx out of range")
+        if not self._sets and n:
+            raise EllipticError("key set is closed")
+        status = np.empty(n, np.uint8)
+        # one native set per wire format: each gets its own items' DER blob and offsets
+        where = self._where[key_idx] if len(self._sets) > 1 else None
+        for k, h in enumerate(self._sets):
+            sel = np.arange(n) if where is None else np.nonzero(where[:, 0] == k)[0]
+            if not len(sel):
+                continue
+            blob, off = _blob([ders[i] for i in sel])
+            idx = key_idx if where is None else where[sel, 1]
+            part = np.empty(len(sel), np.uint8)
+            nat.call(lib.eb200_ecdsa_verify_batch_keyed_der, h, len(sel), np.ascontiguousarray(e[sel]), blob, off,
+                     np.ascontiguousarray(idx, np.uint32), part)
+            status[sel] = part
+        return status
+
     def mul_batch_packed(self, k, key_idx):
         """pub.mul(k) for key key_idx[i] of the set (eb200_scalar_mul_batch_keyed): k is an (n, len) uint8 array, any
         value below 2^(8 len).  Returns ((n, 2 len) x || y big-endian, statuses) as EC.mul_batch's call leaves them."""

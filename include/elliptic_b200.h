@@ -47,6 +47,7 @@ extern "C" {
 #define EB200_ST_RETRY 10               /* (sign with caller nonces) the reference's loop `continue`s: k outside [2, n-2], r = 0 or s = 0;
                                            the caller supplies its next k(iter), ec/index.js:153-185 */
 #define EB200_ST_THROW_NO_RECOVERY 11   /* (getKeyRecoveryParam) threw Error('Unable to find valid recovery factor')  ec/index.js:277 */
+#define EB200_ST_BAD_KEY_INDEX 12       /* (device-pointer keyed calls) key_idx[i] >= m: nothing was computed for the item */
 
 /* curve ids (names of lib/elliptic/curves.js presets) */
 #define EB200_CURVE_SECP256K1 1
@@ -304,9 +305,40 @@ int eb200_keyset_destroy(eb200_keyset* ks);          /* NULL is a no-op returnin
  * first, then TRUE / FALSE, and for an off-curve key the reference's schedule-dependent answer, replayed on the GPU from
  * the key's coordinates.  A key_idx[i] >= m returns EB200_ERR_ARG before anything is written.
  * eb200_last_timing: main_kernel_ms = the keyed main kernel; launches = 3 per chunk (prep, main, replay).
- * There is no device-pointer (`_dev`) and no DER variant of this call yet. */
+ * The same call takes DER signatures (eb200_ecdsa_verify_batch_keyed_der) and device pointers on the caller's stream
+ * (eb200_ecdsa_verify_batch_keyed_dev), below. */
 int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r,
                                    const uint8_t* s, const uint32_t* key_idx, uint8_t* status);
+
+/* Keyed verify of DER signatures off the wire, parsed on the GPU: e, sigs and sig_off as eb200_ecdsa_verify_batch_der
+ * takes them (n + 1 absolute offsets).  status[i] is exactly the byte eb200_ecdsa_verify_batch_der writes for the same e
+ * and DER with pub[i] = key key_idx[i] in the set's format; the first of these that applies: the key's import throw
+ * (keyFromPublic runs before new Signature, ec/index.js:194-195), THROW_SIG_FORMAT for an encoding _importDER rejects,
+ * FALSE for r or s out of range, then the keyed verify's TRUE / FALSE (for an off-curve key, the keyed replay's answer).
+ * An EdDSA, signing or curve25519 set, a NULL pointer, decreasing offsets or a key_idx[i] >= m returns EB200_ERR_ARG;
+ * a set released by eb200_shutdown EB200_ERR_NOT_INIT; both before anything is written.  n = 0 returns EB200_OK.
+ * Host pointers, sharded over the set's devices and chunked with copy / compute overlap as eb200_ecdsa_verify_batch_keyed.
+ * eb200_last_timing: main_kernel_ms = the keyed main kernel; launches = 5 per chunk (keyed DER decode, prep, keyed main,
+ * keyed replay, verdict merge). */
+int eb200_ecdsa_verify_batch_keyed_der(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* sigs,
+                                       const uint64_t* sig_off, const uint32_t* key_idx, uint8_t* status);
+
+/* Keyed verify with DEVICE pointers (e, r, s: n x len; key_idx: n words; status: n bytes) on a caller-supplied CUDA
+ * stream (cudaStream_t cast to void*; NULL = the CUDA default stream), on the device that owns d_status.  Asynchronous,
+ * as eb200_ecdsa_verify_batch_dev: the caller synchronises the stream.  d_workspace must hold
+ * eb200_ecdsa_verify_keyed_workspace_bytes(ks, n) bytes of device memory on that device (0 for NULL or a set that is not
+ * an ECDSA set).  For d_key_idx[i] < m, d_status[i] is exactly what eb200_ecdsa_verify_batch_keyed writes; an index >= m
+ * cannot be refused before launch without synchronising the caller's stream, so its item gets EB200_ST_BAD_KEY_INDEX
+ * and the index never addresses the set.  Returned before any launch: EB200_ERR_ARG for an EdDSA, signing or
+ * curve25519 set, a NULL pointer, or d_status on an initialised device that does not hold this set (one added after
+ * the set was created); EB200_ERR_NOT_INIT for a set released by eb200_shutdown or d_status on a device eb200_init has
+ * not set up.  n = 0 returns EB200_OK.
+ * eb200_last_timing (after the caller has synchronised the stream): kernel_ms = the whole call, main_kernel_ms = the keyed
+ * main kernel; launches = 5 (index screen, prep, keyed main, keyed replay, verdict merge). */
+size_t eb200_ecdsa_verify_keyed_workspace_bytes(const eb200_keyset* ks, size_t n);
+int eb200_ecdsa_verify_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_e, const uint8_t* d_r,
+                                       const uint8_t* d_s, const uint32_t* d_key_idx, uint8_t* d_status,
+                                       void* d_workspace, void* stream);
 
 /* Point.mul / G.mulAdd / KeyPair.derive against the keys of a set (`pub = key.getPublic(); pub.precompute()` once, then
  * `pub.mul(k)`, `G.mulAdd(k1, pub, k2)`, `keyPair.derive(pub)` many times; curve/short.js:422-441, ec/key.js:102-107):
