@@ -16,7 +16,7 @@ OK, ERR_NO_DEVICE, ERR_CUDA, ERR_ARG, ERR_NOT_INIT, ERR_UNSUPPORTED = 0, -1, -2,
 ST_FALSE, ST_TRUE, ST_THROW_INVALID_POINT, ST_THROW_NOT_VALIDATED, ST_NEEDS_HOST, ST_THROW_ASSERT, \
     ST_THROW_POINT_FORMAT = range(7)
 ST_INFINITY, ST_THROW_SECOND_KEY, ST_THROW_SIG_FORMAT, ST_RETRY, ST_THROW_NO_RECOVERY = 7, 8, 9, 10, 11
-ST_BAD_KEY_INDEX = 12
+ST_BAD_KEY_INDEX, ST_BAD_ITEM = 12, 13
 CURVE_SECP256K1, CURVE_P256, CURVE_P384, CURVE_ED25519, CURVE_CURVE25519, CURVE_P521, CURVE_P192, CURVE_P224 = 1, 2, 3, 4, 5, 6, 7, 8
 PUB_XY, PUB_SEC1_65, PUB_SEC1_33 = 0, 1, 2
 KEYSET_MIN_BITS, KEYSET_MAX_BITS, KEYSET_DEFAULT_BUDGET = 4, 8, 1 << 30
@@ -38,6 +38,9 @@ EXPORTS = [
     "eb200_eddsa_signing_set_create", "eb200_eddsa_sign_batch_keyed", "eb200_ecdsa_recovery_param_batch_keyed",
     "eb200_x25519_keyset_create", "eb200_x25519_derive_batch_keyed",
     "eb200_ecdsa_verify_batch_keyed_der", "eb200_ecdsa_verify_keyed_workspace_bytes", "eb200_ecdsa_verify_batch_keyed_dev",
+    "eb200_keyset_dev_workspace_bytes", "eb200_scalar_mul_batch_keyed_dev", "eb200_mul_add_batch_keyed_dev",
+    "eb200_ecdh_derive_batch_keyed_dev", "eb200_ecdsa_recovery_param_batch_keyed_dev", "eb200_eddsa_verify_batch_keyed_dev",
+    "eb200_eddsa_verify_batch_keyed_msgs_dev", "eb200_eddsa_sign_batch_keyed_dev", "eb200_x25519_derive_batch_keyed_dev",
 ]
 
 
@@ -111,6 +114,17 @@ def load():
     lib.eb200_ecdsa_verify_keyed_workspace_bytes.restype = c.c_size_t
     lib.eb200_ecdsa_verify_keyed_workspace_bytes.argtypes = [c.c_void_p, c.c_size_t]
     lib.eb200_ecdsa_verify_batch_keyed_dev.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 7
+    lib.eb200_keyset_dev_workspace_bytes.restype = c.c_size_t
+    lib.eb200_keyset_dev_workspace_bytes.argtypes = [c.c_void_p, c.c_size_t]
+    lib.eb200_scalar_mul_batch_keyed_dev.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 6
+    lib.eb200_mul_add_batch_keyed_dev.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 7
+    lib.eb200_ecdh_derive_batch_keyed_dev.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 6
+    lib.eb200_ecdsa_recovery_param_batch_keyed_dev.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 8
+    lib.eb200_eddsa_verify_batch_keyed_dev.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 7
+    lib.eb200_eddsa_verify_batch_keyed_msgs_dev.argtypes = [c.c_void_p, c.c_size_t, c.c_void_p, c.c_void_p, c.c_void_p,
+                                                            c.c_uint64] + [c.c_void_p] * 5
+    lib.eb200_eddsa_sign_batch_keyed_dev.argtypes = [c.c_void_p, c.c_size_t, c.c_void_p, c.c_uint64] + [c.c_void_p] * 6
+    lib.eb200_x25519_derive_batch_keyed_dev.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 6
     lib.eb200_scalar_mul_batch_keyed.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 4
     lib.eb200_mul_add_batch_keyed.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 5
     lib.eb200_ecdh_derive_batch_keyed.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 4

@@ -2267,23 +2267,59 @@ int verify_keyed_der_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t*
     });
 }
 
-// workspace of eb200_ecdsa_verify_batch_keyed_dev: [screened key_idx (n words) | verdicts (n bytes) | prep words and the
-// inversion scratch, as ws_layout places them]
+// workspace of the keyed device-pointer calls: [screened key_idx (n words) | verdicts (n bytes) | body bytes], the body
+// as each call places it (eb200_ecdsa_verify_batch_keyed_dev: prep words and the inversion scratch, as ws_layout
+// places them)
 struct KeyedDevWs { size_t idx, verdict, prep, total; };
-KeyedDevWs keyed_dev_ws(int curve, size_t n) {
+KeyedDevWs keyed_dev_ws(size_t n, size_t body) {
   KeyedDevWs L;
   L.idx = 0;
   L.verdict = align256(n * 4);
   L.prep = L.verdict + align256(n);
-  L.total = L.prep + ws_layout(curve, n).qtab;
+  L.total = L.prep + body;
   return L;
+}
+
+// Workspace of one keyed mul / mulAdd / derive or getKeyRecoveryParam launch of n items: prep words | inversion scratch
+// (as ws_layout places them) | Jacobian results (3 x limbs x n words; recovery parameter: Y, Z, 2 x limbs x n).
+size_t keyed_mul_ws_bytes(int curve, size_t n) {
+  return align256(ws_layout(curve, n).qtab + 3 * (size_t)keyset_geom(curve).limbs * n * 4);
+}
+
+// The launches of one keyed mul / mulAdd / derive block whose inputs are on the device (k1 == NULL: no base-point term):
+// prep_scalars, keyed main (between ev0 and ev1), normalisation, then the keyed replay (derive: the status map).
+// base: keyed_mul_ws_bytes(curve, m) of workspace.
+int keyed_mul_launches(Ctx& c, int curve, size_t m, const KeysetDev& d, const uint8_t* k1, const uint8_t* k2, const u32* idx,
+                       uint8_t* base, uint8_t* out, uint8_t* status, bool derive, Launch& L, cudaEvent_t ev0, cudaEvent_t ev1) {
+  const WsLayout W = ws_layout(curve, m);
+  u32 *ws = (u32*)(base + W.ws), *scratch = (u32*)(base + W.scratch), *jac = (u32*)(base + W.qtab);
+  const u32* replay = nullptr;
+  int batch = 0;
+  int rc = with_curve(curve, [&](auto cv) {
+    typedef decltype(cv) T;
+    if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;
+    else if constexpr (is_k256<T>) {
+      L(k256_prep_scalars_kernel, blocks128(m), 128, m, k1, k2, ws);
+      replay = c.replay_tab;
+      batch = k256_prep_batch(m);
+    } else {
+      L(sw_prep_scalars_kernel<typename T::C>, blocks128(m), 128, m, k1, k2, ws);
+      replay = c.sw_replay_tab[curve];
+    }
+    return L.rc;
+  });
+  if (rc) return rc;
+  const KeyedMulArgs a{k1, k2, idx, ws, jac, scratch, c.gtab[curve], replay, out, status, batch, derive};
+  cudaError_t err = keyset_mul_launch(curve, m, d, a, L.st, ev0, ev1, &L.count);
+  if (err != cudaSuccess) return cuda_fail(err, "keyset_mul_launch");
+  if (derive) L(status_map_kernel, blocks128(m), 128, m, status, (uint8_t)ST_NEEDS_HOST, (uint8_t)ST_THROW_NOT_VALIDATED);
+  return L.rc;
 }
 
 // Keyed Point.mul / G.mulAdd / KeyPair.derive of one block on one device of the set, chunked like verify_keyed_on.
 // k1 == NULL: k2 times the key (derive: x only, and an off-curve key is THROW_NOT_VALIDATED instead of replayed);
-// else k1 G + k2 times the key.  Launches per chunk: prep_scalars, keyed main, normalisation, then the keyed replay
-// (derive: the status map).  derive: the private scalars, their digit words and the Jacobian results are cleared on
-// the chunk's stream behind its kernels, as x25519_on does.
+// else k1 G + k2 times the key.  Launches per chunk: keyed_mul_launches.  derive: the private scalars, their digit
+// words and the Jacobian results are cleared on the chunk's stream behind its kernels, as x25519_on does.
 int mul_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* k1, const uint8_t* k2, const u32* key_idx,
                  uint8_t* out, uint8_t* status, bool derive) {
   const int curve = ks->curve;
@@ -2291,12 +2327,11 @@ int mul_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* k1, co
   if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
   int rc = ensure_table(c, curve);
   if (rc) return rc;
-  const size_t len = curve_len(curve), ol = derive ? len : 2 * len, limbs = (size_t)keyset_geom(curve).limbs;
+  const size_t len = curve_len(curve), ol = derive ? len : 2 * len;
   const ChunkPlan P = make_plan(n);
   const size_t idx_bytes = align256(n * 4), k_bytes = align256(n * len);
   if ((rc = grow(&c.d_in, &c.d_in_cap, idx_bytes + 2 * k_bytes + n * ol + 256))) return rc;
-  const WsLayout W = ws_layout(curve, P.max_m);
-  const size_t ws_slot = align256(W.qtab + 3 * limbs * P.max_m * 4);   // prep words | inversion scratch | Jacobian results
+  const size_t ws_slot = keyed_mul_ws_bytes(curve, P.max_m);
   if ((rc = grow(&c.d_ws, &c.d_ws_cap, (P.chunks > 1 ? 2 : 1) * ws_slot))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
   u32* d_idx = (u32*)c.d_in;
@@ -2310,30 +2345,10 @@ int mul_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* k1, co
     },
     [&](size_t lo, size_t m, Launch& L, int slot, int k) {
       uint8_t* base = c.d_ws + (size_t)slot * ws_slot;
-      u32 *ws = (u32*)(base + W.ws), *scratch = (u32*)(base + W.scratch), *jac = (u32*)(base + W.qtab);
-      const uint8_t* dk1 = k1 ? d_k1 + lo * len : nullptr;
-      const u32* replay = nullptr;
-      int batch = 0;
-      int rc2 = with_curve(curve, [&](auto cv) {
-        typedef decltype(cv) T;
-        if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;
-        else if constexpr (is_k256<T>) {
-          L(k256_prep_scalars_kernel, blocks128(m), 128, m, dk1, d_k2 + lo * len, ws);
-          replay = c.replay_tab;
-          batch = k256_prep_batch(m);
-        } else {
-          L(sw_prep_scalars_kernel<typename T::C>, blocks128(m), 128, m, dk1, d_k2 + lo * len, ws);
-          replay = c.sw_replay_tab[curve];
-        }
-        return L.rc;
-      });
+      int rc2 = keyed_mul_launches(c, curve, m, d, k1 ? d_k1 + lo * len : nullptr, d_k2 + lo * len, d_idx + lo, base,
+                                   d_out + lo * ol, c.d_status + lo, derive, L, c.ev_k0[k], c.ev_k1[k]);
       if (rc2) return rc2;
-      const KeyedMulArgs a{dk1, d_k2 + lo * len, d_idx + lo, ws, jac, scratch, c.gtab[curve], replay, d_out + lo * ol,
-                           c.d_status + lo, batch, derive};
-      cudaError_t err = keyset_mul_launch(curve, m, d, a, L.st, c.ev_k0[k], c.ev_k1[k], &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "keyset_mul_launch");
       if (derive) {
-        L(status_map_kernel, blocks128(m), 128, m, c.d_status + lo, (uint8_t)ST_NEEDS_HOST, (uint8_t)ST_THROW_NOT_VALIDATED);
         CK(cudaMemsetAsync(d_k2 + lo * len, 0, m * len, L.st));     // the private scalars
         CK(cudaMemsetAsync(base, 0, ws_slot, L.st));                 // their digit words and the Jacobian results
       }
@@ -2346,8 +2361,24 @@ int mul_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* k1, co
     });
 }
 
-// Keyed getKeyRecoveryParam of one block on one device of the set, chunked like mul_keyed_on.  Launches per chunk: the
-// unkeyed recovery-parameter prep (recovery_param.cu), keyed main, recid normalisation, cold (keyset_recovery_param.cu).
+// The launches of one keyed getKeyRecoveryParam block whose inputs are on the device: the unkeyed recovery-parameter
+// prep (recovery_param.cu), keyed main (between ev0 and ev1), recid normalisation, cold (keyset_recovery_param.cu).
+// base: the prep words, inversion scratch and Y, Z as recovery_param_keyed_on places them.
+int keyed_rp_launches(Ctx& c, int curve, size_t m, const KeysetDev& d, const uint8_t* e, const uint8_t* r, const uint8_t* s,
+                      const u32* idx, uint8_t* base, uint8_t* recid, uint8_t* status, Launch& L, cudaEvent_t ev0,
+                      cudaEvent_t ev1) {
+  const WsLayout W = ws_layout(curve, m);
+  u32 *ws = (u32*)(base + W.ws), *scratch = (u32*)(base + W.scratch), *yz = (u32*)(base + W.qtab);
+  cudaError_t err = recovery_param_prep_launch(curve, m, e, r, s, ws, scratch, L.st, &L.count);
+  if (err != cudaSuccess) return cuda_fail(err, "recovery_param_prep_launch");
+  const KeyedRecoveryParamArgs a{e, r, idx, ws, yz, scratch, c.gtab[curve], recid, status,
+                                 curve == EB200_CURVE_SECP256K1 ? k256_prep_batch(m) : 0};
+  err = keyset_recovery_param_launch(curve, m, d, a, L.st, ev0, ev1, &L.count);
+  return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_recovery_param_launch");
+}
+
+// Keyed getKeyRecoveryParam of one block on one device of the set, chunked like mul_keyed_on.  Launches per chunk:
+// keyed_rp_launches.
 int recovery_param_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
                             const u32* key_idx, uint8_t* out_recid, uint8_t* status) {
   const int curve = ks->curve;
@@ -2374,15 +2405,8 @@ int recovery_param_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint
       return 4;
     },
     [&](size_t lo, size_t m, Launch& L, int slot, int k) {
-      uint8_t* base = c.d_ws + (size_t)slot * ws_slot;
-      u32 *ws = (u32*)(base + W.ws), *scratch = (u32*)(base + W.scratch), *yz = (u32*)(base + W.qtab);
-      cudaError_t err = recovery_param_prep_launch(curve, m, d_e + lo * len, d_r + lo * len, d_s + lo * len, ws, scratch, L.st,
-                                                   &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "recovery_param_prep_launch");
-      const KeyedRecoveryParamArgs a{d_e + lo * len, d_r + lo * len, d_idx + lo, ws, yz, scratch, c.gtab[curve], d_id + lo,
-                                     c.d_status + lo, curve == EB200_CURVE_SECP256K1 ? k256_prep_batch(m) : 0};
-      err = keyset_recovery_param_launch(curve, m, d, a, L.st, c.ev_k0[k], c.ev_k1[k], &L.count);
-      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_recovery_param_launch");
+      return keyed_rp_launches(c, curve, m, d, d_e + lo * len, d_r + lo * len, d_s + lo * len, d_idx + lo,
+                               c.d_ws + (size_t)slot * ws_slot, d_id + lo, c.d_status + lo, L, c.ev_k0[k], c.ev_k1[k]);
     },
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {out_recid + lo, d_id + lo, m};
@@ -2630,6 +2654,72 @@ int keyset_create_on_devices(eb200_keyset* ks, eb200_keyset** out, Build&& build
   *out = ks;
   return EB200_OK;
 }
+// ---- device-pointer forms of the keyed calls ---------------------------------------------------------------------------
+// The kinds of set the keyed calls take.
+enum KeyedKind { KK_ECDSA, KK_ED_PUBLIC, KK_ED_SIGNING, KK_X25519 };
+bool keyed_kind_is(const eb200_keyset* ks, KeyedKind k) {
+  switch (k) {
+    case KK_ECDSA: return keyset_geom(ks->curve).limbs != 0;
+    case KK_ED_PUBLIC: return ks->curve == EB200_CURVE_ED25519 && ks->kind == KS_PUBLIC;
+    case KK_ED_SIGNING: return ks->curve == EB200_CURVE_ED25519 && ks->kind == KS_SIGNING;
+    default: return ks->curve == EB200_CURVE_CURVE25519;
+  }
+}
+
+// Body bytes of the workspace (keyed_dev_ws) of the device-pointer calls a set takes, n items:
+//   ECDSA sets: keyed_mul_ws_bytes -- mul / mulAdd / derive and getKeyRecoveryParam as their host forms place it in
+//     each chunk's slot, the keyed verify its prep words and inversion scratch at the start;
+//   EdDSA sets: gathered key bytes (32 n, raw messages only) | h (32 n: the hash, or the screened copies of h);
+//   signing sets: ed_signset_ws_bytes, the sign launch's workspace;
+//   curve25519 sets: screened private scalars (32 n) | x25519_keyset_ws_bytes, the derive launch's workspace.
+size_t keyed_dev_body_bytes(const eb200_keyset* ks, size_t n) {
+  if (keyset_geom(ks->curve).limbs) return keyed_mul_ws_bytes(ks->curve, n);
+  if (ks->curve == EB200_CURVE_CURVE25519) return align256(32 * n) + x25519_keyset_ws_bytes(n);
+  if (ks->kind == KS_SIGNING) return ed_signset_ws_bytes(n);
+  return align256(32 * n) + 32 * n;
+}
+
+// The checks of a keyed device-pointer call, in order: the set's kind, its lifetime, n = 0, the pointers, the device
+// that owns d_status.  Then run(c, L, d, idx, verdict, body) on the caller's stream, with d the set's copy on that
+// device and the workspace's regions as keyed_dev_ws places them.
+template <class Run>
+int keyed_dev_run(const eb200_keyset* ks, KeyedKind kind, size_t n, bool ptrs_ok, uint8_t* d_status, void* d_workspace,
+                  void* stream, Run&& run) {
+  if (!ks || !keyed_kind_is(ks, kind)) return EB200_ERR_ARG;
+  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (n == 0) return EB200_OK;
+  if (!ptrs_ok || !d_status || !d_workspace) return EB200_ERR_ARG;
+  const Ctx* owner = ctx_of(d_status);
+  if (!owner) return EB200_ERR_NOT_INIT;
+  const KeysetDev& d = ks->dev[owner->device];
+  if (!d.tab) return EB200_ERR_ARG;                // an initialised device that does not hold this set
+  const int table = kind == KK_ECDSA ? ks->curve : kind == KK_X25519 ? 0 : EB200_CURVE_ED25519;
+  const KeyedDevWs Lw = keyed_dev_ws(n, 0);
+  uint8_t* base = (uint8_t*)d_workspace;
+  return run_dev(d_status, table, stream, [&](Ctx& c, Launch& L) {
+    return run(c, L, d, (u32*)(base + Lw.idx), base + Lw.verdict, base + Lw.prep);
+  });
+}
+
+// Keyed mul / mulAdd / derive with device pointers: index screen, keyed_mul_launches, merge; derive clears the digit
+// words and Jacobian results behind them.
+int mul_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_k1, const uint8_t* d_k2, const uint32_t* d_key_idx,
+                  uint8_t* d_out, uint8_t* d_status, void* d_workspace, void* stream, bool need_k1, bool derive) {
+  return keyed_dev_run(ks, KK_ECDSA, n, d_k2 && (d_k1 || !need_k1) && d_key_idx && d_out, d_status, d_workspace, stream,
+    [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
+      const int curve = ks->curve;
+      const size_t ol = derive ? curve_len(curve) : 2 * curve_len(curve);
+      cudaError_t err = keyset_index_screen_launch(n, d_key_idx, ks->m, idx, vd, L.st, &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_screen_launch");
+      int rc = keyed_mul_launches(c, curve, n, d, d_k1, d_k2, idx, body, d_out, d_status, derive, L, c.ev[EV_MAIN_BEGIN],
+                                  c.ev[EV_MAIN_END]);
+      if (rc) return rc;
+      if ((err = keyset_verdict_merge_out_launch(n, vd, d_status, d_out, (u32)ol, L.st, &L.count)) != cudaSuccess)
+        return cuda_fail(err, "keyset_verdict_merge_out_launch");
+      if (derive) CK(cudaMemsetAsync(body, 0, keyed_mul_ws_bytes(curve, n), L.st));   // digit words, Jacobian results
+      return EB200_OK;
+    });
+}
 }  // namespace
 
 static void keysets_release_all() {
@@ -2705,41 +2795,30 @@ int eb200_ecdsa_verify_batch_keyed_der(const eb200_keyset* ks, size_t n, const u
 
 size_t eb200_ecdsa_verify_keyed_workspace_bytes(const eb200_keyset* ks, size_t n) {
   if (!ks || !keyset_geom(ks->curve).limbs) return 0;
-  return keyed_dev_ws(ks->curve, n).total;
+  return keyed_dev_ws(n, ws_layout(ks->curve, n).qtab).total;
 }
 
 int eb200_ecdsa_verify_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_e, const uint8_t* d_r,
                                        const uint8_t* d_s, const uint32_t* d_key_idx, uint8_t* d_status,
                                        void* d_workspace, void* stream) {
-  if (!ks || !keyset_geom(ks->curve).limbs) return EB200_ERR_ARG;
-  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!d_e || !d_r || !d_s || !d_key_idx || !d_status || !d_workspace) return EB200_ERR_ARG;
-  const Ctx* owner = ctx_of(d_status);
-  if (!owner) return EB200_ERR_NOT_INIT;
-  const KeysetDev& d = ks->dev[owner->device];
-  if (!d.tab) return EB200_ERR_ARG;                // an initialised device that does not hold this set
-  const int curve = ks->curve;
-  return run_dev(d_status, curve, stream, [&](Ctx& c, Launch& L) {
-    const KeyedDevWs Lw = keyed_dev_ws(curve, n);
-    const WsLayout W = ws_layout(curve, n);
-    uint8_t* base = (uint8_t*)d_workspace;
-    u32* idx = (u32*)(base + Lw.idx);
-    uint8_t* vd = base + Lw.verdict;
-    u32* ws = (u32*)(base + Lw.prep + W.ws);
-    u32* scratch = (u32*)(base + Lw.prep + W.scratch);
-    cudaError_t err = keyset_index_screen_launch(n, d_key_idx, ks->m, idx, vd, L.st, &L.count);
-    if (err != cudaSuccess) return cuda_fail(err, "keyset_index_screen_launch");
-    const u32* replay = nullptr;
-    int rc = keyed_verify_prep(c, curve, n, d_e, d_r, d_s, ws, scratch, L, &replay);
-    if (rc) return rc;
-    const KeyedVerifyArgs a{d_e, d_r, d_s, idx, d_status, ws, c.gtab[curve], replay};
-    if ((err = keyset_verify_launch(curve, n, d, a, L.st, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END], &L.count)) != cudaSuccess)
-      return cuda_fail(err, "keyset_verify_launch");
-    if ((err = keyset_verdict_merge_launch(n, vd, d_status, L.st, &L.count)) != cudaSuccess)
-      return cuda_fail(err, "keyset_verdict_merge_launch");
-    return EB200_OK;
-  });
+  return keyed_dev_run(ks, KK_ECDSA, n, d_e && d_r && d_s && d_key_idx, d_status, d_workspace, stream,
+    [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
+      const int curve = ks->curve;
+      const WsLayout W = ws_layout(curve, n);
+      u32* ws = (u32*)(body + W.ws);
+      u32* scratch = (u32*)(body + W.scratch);
+      cudaError_t err = keyset_index_screen_launch(n, d_key_idx, ks->m, idx, vd, L.st, &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_screen_launch");
+      const u32* replay = nullptr;
+      int rc = keyed_verify_prep(c, curve, n, d_e, d_r, d_s, ws, scratch, L, &replay);
+      if (rc) return rc;
+      const KeyedVerifyArgs a{d_e, d_r, d_s, idx, d_status, ws, c.gtab[curve], replay};
+      if ((err = keyset_verify_launch(curve, n, d, a, L.st, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END], &L.count)) != cudaSuccess)
+        return cuda_fail(err, "keyset_verify_launch");
+      if ((err = keyset_verdict_merge_launch(n, vd, d_status, L.st, &L.count)) != cudaSuccess)
+        return cuda_fail(err, "keyset_verdict_merge_launch");
+      return EB200_OK;
+    });
 }
 
 }  // extern "C"
@@ -2878,6 +2957,134 @@ int eb200_x25519_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint
   return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
     return x25519_derive_keyed_on(c, ks, m, priv + 32 * lo, key_idx + lo, out_x + 32 * lo, status + lo);
   });
+}
+
+}  // extern "C"
+
+extern "C" {
+
+size_t eb200_keyset_dev_workspace_bytes(const eb200_keyset* ks, size_t n) {
+  if (!ks) return 0;
+  return keyed_dev_ws(n, keyed_dev_body_bytes(ks, n)).total;
+}
+
+int eb200_scalar_mul_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_k, const uint32_t* d_key_idx,
+                                     uint8_t* d_out_xy, uint8_t* d_status, void* d_workspace, void* stream) {
+  return mul_keyed_dev(ks, n, nullptr, d_k, d_key_idx, d_out_xy, d_status, d_workspace, stream, false, false);
+}
+
+int eb200_mul_add_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_k1, const uint8_t* d_k2,
+                                  const uint32_t* d_key_idx, uint8_t* d_out_xy, uint8_t* d_status, void* d_workspace,
+                                  void* stream) {
+  return mul_keyed_dev(ks, n, d_k1, d_k2, d_key_idx, d_out_xy, d_status, d_workspace, stream, true, false);
+}
+
+int eb200_ecdh_derive_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_priv, const uint32_t* d_key_idx,
+                                      uint8_t* d_out_x, uint8_t* d_status, void* d_workspace, void* stream) {
+  return mul_keyed_dev(ks, n, nullptr, d_priv, d_key_idx, d_out_x, d_status, d_workspace, stream, false, true);
+}
+
+int eb200_ecdsa_recovery_param_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_e, const uint8_t* d_r,
+                                               const uint8_t* d_s, const uint32_t* d_key_idx, uint8_t* d_out_recid,
+                                               uint8_t* d_status, void* d_workspace, void* stream) {
+  return keyed_dev_run(ks, KK_ECDSA, n, d_e && d_r && d_s && d_key_idx && d_out_recid, d_status, d_workspace, stream,
+    [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
+      cudaError_t err = keyset_index_screen_launch(n, d_key_idx, ks->m, idx, vd, L.st, &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_screen_launch");
+      int rc = keyed_rp_launches(c, ks->curve, n, d, d_e, d_r, d_s, idx, body, d_out_recid, d_status, L, c.ev[EV_MAIN_BEGIN],
+                                 c.ev[EV_MAIN_END]);
+      if (rc) return rc;
+      if ((err = keyset_verdict_merge_out_launch(n, vd, d_status, d_out_recid, 1, L.st, &L.count)) != cudaSuccess)
+        return cuda_fail(err, "keyset_verdict_merge_out_launch");
+      return EB200_OK;
+    });
+}
+
+// workspace body: [unused (32 n) | screened h (32 n)]
+int eb200_eddsa_verify_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_R, const uint8_t* d_S,
+                                       const uint8_t* d_h, const uint32_t* d_key_idx, uint8_t* d_status, void* d_workspace,
+                                       void* stream) {
+  return keyed_dev_run(ks, KK_ED_PUBLIC, n, d_R && d_S && d_h && d_key_idx, d_status, d_workspace, stream,
+    [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
+      uint8_t* h = body + align256(32 * n);
+      cudaError_t err = keyset_index_scalar_screen_launch(n, d_key_idx, ks->m, d_h, false, idx, h, vd, L.st, &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_scalar_screen_launch");
+      CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
+      if ((err = ed_keyset_verify_launch(n, d, d_R, d_S, h, idx, c.gtab[EB200_CURVE_ED25519], d_status, L.st, &L.count)) !=
+          cudaSuccess)
+        return cuda_fail(err, "ed_keyset_verify_launch");
+      CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
+      if ((err = keyset_verdict_merge_launch(n, vd, d_status, L.st, &L.count)) != cudaSuccess)
+        return cuda_fail(err, "keyset_verdict_merge_launch");
+      return EB200_OK;
+    });
+}
+
+// workspace body: [gathered key bytes (32 n) | h (32 n)]
+int eb200_eddsa_verify_batch_keyed_msgs_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_R, const uint8_t* d_S,
+                                            const uint8_t* d_msgs, uint64_t msgs_len, const uint64_t* d_msg_off,
+                                            const uint32_t* d_key_idx, uint8_t* d_status, void* d_workspace, void* stream) {
+  return keyed_dev_run(ks, KK_ED_PUBLIC, n, d_R && d_S && d_msg_off && d_key_idx && (d_msgs || !msgs_len), d_status,
+                       d_workspace, stream,
+    [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
+      uint8_t *A = body, *h = body + align256(32 * n);
+      cudaError_t err = keyset_index_range_screen_launch(n, d_key_idx, ks->m, d_msg_off, msgs_len, idx, vd, L.st, &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_range_screen_launch");
+      if ((err = ed_keyset_gather_launch(n, d, idx, A, L.st, &L.count)) != cudaSuccess)
+        return cuda_fail(err, "ed_keyset_gather_launch");
+      if ((err = keyset_ed_hash_screened_launch(n, vd, d_R, A, d_msgs, d_msg_off, h, L.st, &L.count)) != cudaSuccess)
+        return cuda_fail(err, "keyset_ed_hash_screened_launch");
+      CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
+      if ((err = ed_keyset_verify_launch(n, d, d_R, d_S, h, idx, c.gtab[EB200_CURVE_ED25519], d_status, L.st, &L.count)) !=
+          cudaSuccess)
+        return cuda_fail(err, "ed_keyset_verify_launch");
+      CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
+      if ((err = keyset_verdict_merge_launch(n, vd, d_status, L.st, &L.count)) != cudaSuccess)
+        return cuda_fail(err, "keyset_verdict_merge_launch");
+      return EB200_OK;
+    });
+}
+
+// workspace body: the sign launch's (ed_signset_ws_bytes); its nonces are cleared behind the kernels, as
+// eddsa_sign_keyed_on clears them
+int eb200_eddsa_sign_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_msgs, uint64_t msgs_len,
+                                     const uint64_t* d_msg_off, const uint32_t* d_key_idx, uint8_t* d_out_sig,
+                                     uint8_t* d_status, void* d_workspace, void* stream) {
+  return keyed_dev_run(ks, KK_ED_SIGNING, n, d_msg_off && d_key_idx && d_out_sig && (d_msgs || !msgs_len), d_status,
+                       d_workspace, stream,
+    [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
+      cudaError_t err = keyset_index_range_screen_launch(n, d_key_idx, ks->m, d_msg_off, msgs_len, idx, vd, L.st, &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_range_screen_launch");
+      if ((err = keyset_ss_sign_screened_launch(n, vd, d, d_msgs, d_msg_off, idx, c.gtab[EB200_CURVE_ED25519], (u32*)body,
+                                                d_out_sig, L.st, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END], &L.count)) !=
+          cudaSuccess)
+        return cuda_fail(err, "keyset_ss_sign_screened_launch");
+      CK(cudaMemsetAsync(d_status, EB200_ST_TRUE, n, L.st));          // the reference cannot fail here
+      if ((err = keyset_verdict_merge_out_launch(n, vd, d_status, d_out_sig, 64, L.st, &L.count)) != cudaSuccess)
+        return cuda_fail(err, "keyset_verdict_merge_out_launch");
+      CK(cudaMemsetAsync(body + ed_signset_nonce_offset(n), 0, ed_signset_nonce_bytes(n), L.st));   // the nonces r
+      return EB200_OK;
+    });
+}
+
+// workspace body: [screened private scalars (32 n) | the derive launch's (x25519_keyset_ws_bytes)], all cleared behind
+// the kernels
+int eb200_x25519_derive_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_priv, const uint32_t* d_key_idx,
+                                        uint8_t* d_out_x, uint8_t* d_status, void* d_workspace, void* stream) {
+  return keyed_dev_run(ks, KK_X25519, n, d_priv && d_key_idx && d_out_x, d_status, d_workspace, stream,
+    [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
+      uint8_t* k = body;
+      u32* ws = (u32*)(body + align256(32 * n));
+      cudaError_t err = keyset_index_scalar_screen_launch(n, d_key_idx, ks->m, d_priv, true, idx, k, vd, L.st, &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_scalar_screen_launch");
+      if ((err = x25519_keyset_derive_launch(n, d, k, idx, ws, d_out_x, d_status, L.st, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END],
+                                             &L.count)) != cudaSuccess)
+        return cuda_fail(err, "x25519_keyset_derive_launch");
+      if ((err = keyset_verdict_merge_out_launch(n, vd, d_status, d_out_x, 32, L.st, &L.count)) != cudaSuccess)
+        return cuda_fail(err, "keyset_verdict_merge_out_launch");
+      CK(cudaMemsetAsync(body, 0, keyed_dev_body_bytes(ks, n), L.st));   // the scalars and the per-item results
+      return EB200_OK;
+    });
 }
 
 }  // extern "C"

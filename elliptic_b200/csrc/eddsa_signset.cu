@@ -62,6 +62,12 @@ cudaError_t ed_signset_create_launch(size_t m, const KeysetDev& k, const uint8_t
   return cudaSuccess;
 }
 
+cudaError_t ed_signset_normalise_launch(size_t n, uint32_t* ws, uint8_t* sig, cudaStream_t st, unsigned* launches) {
+  ESS_LAUNCH((ed_signset_normalise_kernel<<<blocks_of((n + ED_SS_BATCH - 1) / ED_SS_BATCH, ED_SS_NORM_THREADS),
+                                            ED_SS_NORM_THREADS, 0, st>>>(n, ws, sig)));
+  return cudaSuccess;
+}
+
 size_t ed_signset_ws_bytes(size_t n) { return (size_t)ED_SS_WS_WORDS * 4 * n; }
 size_t ed_signset_nonce_bytes(size_t n) { return (size_t)8 * 4 * n; }
 size_t ed_signset_nonce_offset(size_t n) { return (size_t)ED_SS_WS_R * 4 * n; }
@@ -73,8 +79,7 @@ cudaError_t ed_signset_sign_launch(size_t n, const KeysetDev& k, const uint8_t* 
   if ((err = cudaEventRecord(main_begin, st)) != cudaSuccess) return err;
   ESS_LAUNCH((ed_signset_nonce_kernel<<<blocks_of(n, 128), 128, 0, st>>>(n, msgs, msg_off, key_idx, k.tab, gtab, ws)));
   if ((err = cudaEventRecord(main_end, st)) != cudaSuccess) return err;
-  ESS_LAUNCH((ed_signset_normalise_kernel<<<blocks_of((n + ED_SS_BATCH - 1) / ED_SS_BATCH, ED_SS_NORM_THREADS),
-                                            ED_SS_NORM_THREADS, 0, st>>>(n, ws, sig)));
+  if ((err = ed_signset_normalise_launch(n, ws, sig, st, launches)) != cudaSuccess) return err;
   ESS_LAUNCH((ed_signset_challenge_kernel<<<blocks_of(n, 128), 128, 0, st>>>(n, msgs, msg_off, key_idx, k.tab, k.xy, ws, sig)));
   return cudaSuccess;
 }

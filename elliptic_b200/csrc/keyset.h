@@ -1,5 +1,5 @@
-// keyset.h -- the key-set kernels (keyset.cu, keyset_forms.cu, keyset_mul.cu, keyset_recovery_param.cu, eddsa_keyset.cu,
-// eddsa_signset.cu, x25519_keyset.cu), launched by eb200.cu
+// keyset.h -- the key-set kernels (keyset.cu, keyset_forms.cu, keyset_forms_nonce.cu, keyset_mul.cu,
+// keyset_recovery_param.cu, eddsa_keyset.cu, eddsa_signset.cu, x25519_keyset.cu), launched by eb200.cu
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -55,6 +55,34 @@ cudaError_t keyset_index_screen_launch(size_t n, const uint32_t* key_idx, size_t
                                        cudaStream_t st, unsigned* launches);
 // Verdict merge, behind the keyed replay: status[i] = verdict[i] wherever that is not 0.
 cudaError_t keyset_verdict_merge_launch(size_t n, const uint8_t* verdict, uint8_t* status, cudaStream_t st, unsigned* launches);
+// The device-pointer forms of the other keyed calls (keyset_forms_body.cuh), one kernel each unless stated.
+// Index and scalar screen: as the index screen, and k_out[32 i ..] = the 32-byte scalar k[32 i ..] (little-endian, or
+// big_endian), zeros with verdict EB200_ST_BAD_ITEM when it is not below the ed25519 group order n.
+cudaError_t keyset_index_scalar_screen_launch(size_t n, const uint32_t* key_idx, size_t m, const uint8_t* k, bool big_endian,
+                                              uint32_t* idx_out, uint8_t* k_out, uint8_t* verdict, cudaStream_t st,
+                                              unsigned* launches);
+// Index and range screen: as the index screen, then verdict EB200_ST_BAD_ITEM for off[i + 1] < off[i] or > msgs_len.
+cudaError_t keyset_index_range_screen_launch(size_t n, const uint32_t* key_idx, size_t m, const uint64_t* off,
+                                             uint64_t msgs_len, uint32_t* idx_out, uint8_t* verdict, cudaStream_t st,
+                                             unsigned* launches);
+// Verdict merge of a call with outputs: as the verdict merge, and out[ol i .. ol i + ol) = 0 where the verdict is not 0.
+cudaError_t keyset_verdict_merge_out_launch(size_t n, const uint8_t* verdict, uint8_t* status, uint8_t* out, uint32_t ol,
+                                            cudaStream_t st, unsigned* launches);
+// The keyed EdDSA hash (ed25519_hash_kernel) of the items whose verdict is 0; h = 0 for the others.
+cudaError_t keyset_ed_hash_screened_launch(size_t n, const uint8_t* verdict, const uint8_t* R, const uint8_t* A,
+                                           const uint8_t* msgs, const uint64_t* msg_off, uint8_t* h, cudaStream_t st,
+                                           unsigned* launches);
+// keyset_forms_nonce.cu: the screened nonce kernel alone (one kernel); the items whose verdict is not 0 read no message
+// byte and leave R = the identity, r = 0 in ws.
+cudaError_t keyset_ss_nonce_screened_launch(size_t n, const uint8_t* verdict, const KeysetDev& k, const uint8_t* msgs,
+                                            const uint64_t* msg_off, const uint32_t* key_idx, const uint32_t* gtab,
+                                            uint32_t* ws, cudaStream_t st, unsigned* launches);
+// ed_signset_sign_launch with screened nonce and challenge kernels around the unchanged normalisation: the items whose
+// verdict is not 0 read no message byte and leave R = the identity, r = 0 in ws.  Three kernels.
+cudaError_t keyset_ss_sign_screened_launch(size_t n, const uint8_t* verdict, const KeysetDev& k, const uint8_t* msgs,
+                                           const uint64_t* msg_off, const uint32_t* key_idx, const uint32_t* gtab, uint32_t* ws,
+                                           uint8_t* sig, cudaStream_t st, cudaEvent_t main_begin, cudaEvent_t main_end,
+                                           unsigned* launches);
 
 // keyset_mul.cu.  Device buffers of one keyed mul / mulAdd / derive block: k1 (NULL: no base-point term), k2 (n x len, as the caller
 // gave them: the replay uses them unreduced) and key_idx in; ws as the curve's unkeyed prep_scalars kernel left it;
@@ -123,6 +151,8 @@ size_t ed_signset_nonce_bytes(size_t n);
 cudaError_t ed_signset_sign_launch(size_t n, const KeysetDev& k, const uint8_t* msgs, const uint64_t* msg_off,
                                    const uint32_t* key_idx, const uint32_t* gtab, uint32_t* ws, uint8_t* sig, cudaStream_t st,
                                    cudaEvent_t main_begin, cudaEvent_t main_end, unsigned* launches);
+// The normalisation kernel of a sign launch alone: R of the n items in ws encoded into sig[64 i ..].  One kernel.
+cudaError_t ed_signset_normalise_launch(size_t n, uint32_t* ws, uint8_t* sig, cudaStream_t st, unsigned* launches);
 
 // curve25519 key sets (x25519_keyset.cu).  Build: classifies the m keys (pubx: m x 32 big-endian, on the device), writes
 // their Edwards images to k.xy and builds their tables on `st`; bases: scratch of m * ed_keyset_windows(W) * 24 words.

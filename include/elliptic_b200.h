@@ -48,6 +48,8 @@ extern "C" {
                                            the caller supplies its next k(iter), ec/index.js:153-185 */
 #define EB200_ST_THROW_NO_RECOVERY 11   /* (getKeyRecoveryParam) threw Error('Unable to find valid recovery factor')  ec/index.js:277 */
 #define EB200_ST_BAD_KEY_INDEX 12       /* (device-pointer keyed calls) key_idx[i] >= m: nothing was computed for the item */
+#define EB200_ST_BAD_ITEM 13            /* (device-pointer keyed calls) an argument the host form refuses with EB200_ERR_ARG:
+                                           nothing was computed for the item */
 
 /* curve ids (names of lib/elliptic/curves.js presets) */
 #define EB200_CURVE_SECP256K1 1
@@ -462,6 +464,59 @@ int eb200_x25519_keyset_create(size_t m, const uint8_t* pubx, uint32_t table_bit
  * eb200_last_timing: main_kernel_ms = the keyed main kernel; launches = 2 per chunk. */
 int eb200_x25519_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* priv, const uint32_t* key_idx,
                                     uint8_t* out_x, uint8_t* status);
+
+/* Device-pointer forms of the keyed calls above, for CUDA callers whose data is already on the GPU.  Each takes its host
+ * form's arguments as DEVICE pointers, then d_workspace and a CUDA stream (cudaStream_t cast to void*; NULL = the CUDA
+ * default stream), as eb200_ecdsa_verify_batch_keyed_dev, and runs asynchronously on that stream on the device that owns
+ * d_status; the caller synchronises the stream.  d_workspace must hold eb200_keyset_dev_workspace_bytes(ks, n) bytes of
+ * device memory on that device; the call never reads it before writing it.
+ * Outputs and statuses: for every item whose arguments the host form accepts, byte for byte what the host form writes.
+ * An argument the host form refuses with EB200_ERR_ARG cannot be refused before launch without synchronising the stream,
+ * so the item gets a status instead, its outputs are zeroed and nothing is computed from the bad value (a bad index
+ * never addresses the set, a bad scalar never reaches its tables, a bad range is never read):
+ *   EB200_ST_BAD_KEY_INDEX for d_key_idx[i] >= m; otherwise
+ *   EB200_ST_BAD_ITEM for an EdDSA h >= n (little-endian), a curve25519 priv >= n (big-endian), or a message range with
+ *     d_msg_off[i + 1] < d_msg_off[i] or d_msg_off[i + 1] > msgs_len (d_msg_off: n + 1 offsets into the msgs_len bytes
+ *     at d_msgs, which may be NULL only when msgs_len = 0).
+ * Returned before any launch: EB200_ERR_ARG for a set of another kind (as the host form), a NULL pointer, or d_status
+ * on an initialised device that does not hold the set; EB200_ERR_NOT_INIT for a set released by eb200_shutdown or
+ * d_status on a device eb200_init has not set up.  n = 0 returns EB200_OK.
+ * ECDH derive, curve25519 derive and EdDSA sign clear, on the stream before their work ends, every workspace region that
+ * held scalar-derived data (screened scalar copies, digit words, per-item results, nonces); the caller's own buffers
+ * are the caller's.
+ * eb200_last_timing (after the caller has synchronised the stream): kernel_ms = the whole call, main_kernel_ms = the keyed
+ * main kernel (the nonce kernel for sign); launches as stated per call. */
+size_t eb200_keyset_dev_workspace_bytes(const eb200_keyset* ks, size_t n);   /* 0 for NULL; for an ECDSA set at least
+                                                                                eb200_ecdsa_verify_keyed_workspace_bytes */
+/* ECDSA sets.  launches = 6: index screen, scalar prep, keyed main, normalisation, keyed replay (derive: the status
+ * map), merge. */
+int eb200_scalar_mul_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_k, const uint32_t* d_key_idx,
+                                     uint8_t* d_out_xy, uint8_t* d_status, void* d_workspace, void* stream);
+int eb200_mul_add_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_k1, const uint8_t* d_k2,
+                                  const uint32_t* d_key_idx, uint8_t* d_out_xy, uint8_t* d_status, void* d_workspace,
+                                  void* stream);
+int eb200_ecdh_derive_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_priv, const uint32_t* d_key_idx,
+                                      uint8_t* d_out_x, uint8_t* d_status, void* d_workspace, void* stream);
+/* launches = 6: index screen, prep, keyed main, recid normalisation, cold kernel, merge. */
+int eb200_ecdsa_recovery_param_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_e, const uint8_t* d_r,
+                                               const uint8_t* d_s, const uint32_t* d_key_idx, uint8_t* d_out_recid,
+                                               uint8_t* d_status, void* d_workspace, void* stream);
+/* EdDSA sets.  launches = 3 (index and h screen, keyed main, merge), or 5 for raw messages (index and range screen,
+ * key-byte gather, hash, keyed main, merge). */
+int eb200_eddsa_verify_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_R, const uint8_t* d_S,
+                                       const uint8_t* d_h, const uint32_t* d_key_idx, uint8_t* d_status, void* d_workspace,
+                                       void* stream);
+int eb200_eddsa_verify_batch_keyed_msgs_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_R, const uint8_t* d_S,
+                                            const uint8_t* d_msgs, uint64_t msgs_len, const uint64_t* d_msg_off,
+                                            const uint32_t* d_key_idx, uint8_t* d_status, void* d_workspace, void* stream);
+/* EdDSA signing sets.  d_status[i] = EB200_ST_TRUE for an accepted item.  launches = 5: index and range screen, nonce,
+ * normalisation, challenge, merge. */
+int eb200_eddsa_sign_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_msgs, uint64_t msgs_len,
+                                     const uint64_t* d_msg_off, const uint32_t* d_key_idx, uint8_t* d_out_sig,
+                                     uint8_t* d_status, void* d_workspace, void* stream);
+/* curve25519 sets.  launches = 4: index and priv screen, keyed main, normalisation, merge. */
+int eb200_x25519_derive_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_priv, const uint32_t* d_key_idx,
+                                        uint8_t* d_out_x, uint8_t* d_status, void* d_workspace, void* stream);
 
 /* Self-test hooks used by the parity tests (device arithmetic vs the oracle).
  * a, b, out: n elements of L little-endian 32-bit limbs each (host pointers); L = 8, except p192 6, p384 12 and
