@@ -41,6 +41,10 @@ EXPORTS = [
     "eb200_keyset_dev_workspace_bytes", "eb200_scalar_mul_batch_keyed_dev", "eb200_mul_add_batch_keyed_dev",
     "eb200_ecdh_derive_batch_keyed_dev", "eb200_ecdsa_recovery_param_batch_keyed_dev", "eb200_eddsa_verify_batch_keyed_dev",
     "eb200_eddsa_verify_batch_keyed_msgs_dev", "eb200_eddsa_sign_batch_keyed_dev", "eb200_x25519_derive_batch_keyed_dev",
+    "eb200_dev_workspace_bytes", "eb200_ecdsa_sign_batch_dev", "eb200_ecdsa_sign_batch_k_dev", "eb200_ecdsa_sign_batch_pers_dev",
+    "eb200_ec_keygen_batch_dev", "eb200_ecdsa_recover_batch_dev", "eb200_ecdsa_recovery_param_batch_dev",
+    "eb200_scalar_mul_batch_dev", "eb200_mul_add_batch_dev", "eb200_ecdh_derive_batch_dev", "eb200_x25519_mul_batch_dev",
+    "eb200_ecdsa_verify_batch_der_dev", "eb200_eddsa_verify_batch_msgs_dev", "eb200_eddsa_sign_batch_dev",
 ]
 
 
@@ -125,6 +129,24 @@ def load():
                                                             c.c_uint64] + [c.c_void_p] * 5
     lib.eb200_eddsa_sign_batch_keyed_dev.argtypes = [c.c_void_p, c.c_size_t, c.c_void_p, c.c_uint64] + [c.c_void_p] * 6
     lib.eb200_x25519_derive_batch_keyed_dev.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 6
+    lib.eb200_dev_workspace_bytes.restype = c.c_size_t
+    lib.eb200_dev_workspace_bytes.argtypes = [c.c_int, c.c_size_t]
+    lib.eb200_ecdsa_sign_batch_dev.argtypes = [c.c_int, c.c_size_t, c.c_void_p, c.c_void_p, c.c_uint32] + [c.c_void_p] * 6
+    lib.eb200_ecdsa_sign_batch_k_dev.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 3 + [c.c_uint32] + [c.c_void_p] * 6
+    lib.eb200_ecdsa_sign_batch_pers_dev.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 3 + [c.c_size_t, c.c_uint32] + \
+        [c.c_void_p] * 6
+    lib.eb200_ec_keygen_batch_dev.argtypes = [c.c_int, c.c_size_t, c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t] + \
+        [c.c_void_p] * 5
+    lib.eb200_ecdsa_recover_batch_dev.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 8
+    lib.eb200_ecdsa_recovery_param_batch_dev.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 8
+    lib.eb200_scalar_mul_batch_dev.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 6
+    lib.eb200_mul_add_batch_dev.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 7
+    lib.eb200_ecdh_derive_batch_dev.argtypes = [c.c_int, c.c_size_t] + [c.c_void_p] * 6
+    lib.eb200_x25519_mul_batch_dev.argtypes = [c.c_size_t] + [c.c_void_p] * 5
+    lib.eb200_ecdsa_verify_batch_der_dev.argtypes = [c.c_int, c.c_size_t, c.c_void_p, c.c_void_p, c.c_uint64, c.c_void_p,
+                                                     c.c_void_p, c.c_uint32] + [c.c_void_p] * 3
+    lib.eb200_eddsa_verify_batch_msgs_dev.argtypes = [c.c_size_t] + [c.c_void_p] * 4 + [c.c_uint64] + [c.c_void_p] * 4
+    lib.eb200_eddsa_sign_batch_dev.argtypes = [c.c_size_t, c.c_void_p, c.c_void_p, c.c_uint64] + [c.c_void_p] * 6
     lib.eb200_scalar_mul_batch_keyed.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 4
     lib.eb200_mul_add_batch_keyed.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 5
     lib.eb200_ecdh_derive_batch_keyed.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 4

@@ -9,7 +9,8 @@ SRC = [os.path.join(HERE, "csrc", "eb200.cu"), os.path.join(HERE, "csrc", "recov
        os.path.join(HERE, "csrc", "keyset.cu"), os.path.join(HERE, "csrc", "eddsa_keyset.cu"),
        os.path.join(HERE, "csrc", "keyset_mul.cu"), os.path.join(HERE, "csrc", "eddsa_signset.cu"),
        os.path.join(HERE, "csrc", "keyset_recovery_param.cu"), os.path.join(HERE, "csrc", "x25519_keyset.cu"),
-       os.path.join(HERE, "csrc", "keyset_forms.cu"), os.path.join(HERE, "csrc", "keyset_forms_nonce.cu")]
+       os.path.join(HERE, "csrc", "keyset_forms.cu"), os.path.join(HERE, "csrc", "keyset_forms_nonce.cu"),
+       os.path.join(HERE, "csrc", "unkeyed_forms.cu")]
 DEPS = [os.path.join(HERE, "csrc", f) for f in os.listdir(os.path.join(HERE, "csrc"))] + [
     os.path.join(HERE, "..", "include", "elliptic_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-split-compile", "0",

@@ -27,6 +27,7 @@
 #include "kernel_bounds.h"
 #include "recovery_param.h"
 #include "keyset.h"
+#include "unkeyed_forms.h"
 
 using namespace eb;
 
@@ -894,11 +895,13 @@ int ensure_table(Ctx& c, int curve) {
 }
 
 // Launches decode (if needed) + prep + verify for n items on L's stream, recording ev_main0 / ev_main1 around the
-// main kernel.  All pointers are device pointers.
+// main kernel.  All pointers are device pointers.  der_verdict: a range screen's verdicts, for which the screened DER
+// decode (unkeyed_forms.cu) takes der_decode_kernel's place.
 int launch_verify(Ctx& c, int curve, size_t n, const uint8_t* d_e, const uint8_t* d_r, const uint8_t* d_s,
                   const uint8_t* d_pub, u32 pub_fmt, uint8_t* d_status, uint8_t* d_workspace, Launch& L,
                   cudaEvent_t ev_main0, cudaEvent_t ev_main1,
-                  const uint8_t* d_der = nullptr, const unsigned long long* d_der_off = nullptr) {
+                  const uint8_t* d_der = nullptr, const unsigned long long* d_der_off = nullptr,
+                  const uint8_t* der_verdict = nullptr) {
   if (n == 0) return EB200_OK;
   const WsLayout W = ws_layout(curve, n);
   u32* ws = (u32*)(d_workspace + W.ws);
@@ -918,7 +921,14 @@ int launch_verify(Ctx& c, int curve, size_t n, const uint8_t* d_e, const uint8_t
       else L(sw_decode_pub_kernel<typename T::C>, nb, 128, n, d_pub, pub_fmt, dxy, dpre);
       xy = dxy; pre = dpre;
     }
-    if (d_der) {     // d_r / d_s are then scratch the decoder fills
+    if (d_der && der_verdict) {     // d_r / d_s are then scratch the decoder fills
+      if (L.rc) return L.rc;
+      cudaError_t err = unkeyed_der_decode_screened_launch(n, (u32)curve_len(curve), der_verdict, d_der, d_der_off,
+                                                           (uint8_t*)d_r, (uint8_t*)d_s, dpre, (int)(pre != nullptr), L.st,
+                                                           &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "unkeyed_der_decode_screened_launch");
+      pre = dpre;
+    } else if (d_der) {
       L(der_decode_kernel, nb, 128, n, (u32)curve_len(curve), d_der, d_der_off, (uint8_t*)d_r, (uint8_t*)d_s, dpre,
         (int)(pre != nullptr));
       pre = dpre;
@@ -1376,6 +1386,33 @@ int eb200_ecdsa_verify_batch_der(int curve, size_t n, const uint8_t* e, const ui
 // ---- ECDSA public-key recovery ------------------------------------------------------------
 }  // extern "C"
 
+// The launches of one recoverPubKey block whose inputs are on the device: prep, then the recovery kernel between ev0 and
+// ev1.  base: ws_layout(curve, n).total bytes of workspace.
+static int recover_launches(Ctx& c, int curve, size_t n, const uint8_t* d_e, const uint8_t* d_r, const uint8_t* d_s,
+                            const uint8_t* d_id, uint8_t* base, uint8_t* d_out, uint8_t* d_status, Launch& L, cudaEvent_t ev0,
+                            cudaEvent_t ev1) {
+  const WsLayout W = ws_layout(curve, n);
+  u32 *ws = (u32*)(base + W.ws), *qtab = (u32*)(base + W.qtab);
+  return with_curve(curve, [&](auto cv) {
+    typedef decltype(cv) T;
+    if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;     // the entry points refuse it first
+    else {
+      if constexpr (is_k256<T>) {
+        L(k256_prep_recover_kernel, batch_blocks(n, PREP_BATCH), 128, n, d_e, d_r, d_s, ws, (u32*)(base + W.scratch));
+        CK(cudaEventRecord(ev0, L.st));
+        L(k256_recover_kernel, (unsigned)((n + EB_VERIFY_BLOCK - 1) / EB_VERIFY_BLOCK), EB_VERIFY_BLOCK, n, d_r, d_id, ws,
+          c.gtab[curve], qtab, d_out, d_status);
+      } else {
+        L(sw_prep_recover_kernel<typename T::C>, blocks128(n), 128, n, d_e, d_r, d_s, ws);
+        CK(cudaEventRecord(ev0, L.st));
+        L(sw_recover_kernel<typename T::C>, blocks128(n), 128, n, d_r, d_id, ws, c.gtab[curve], qtab, d_out, d_status);
+      }
+      CK(cudaEventRecord(ev1, L.st));
+      return EB200_OK;
+    }
+  });
+}
+
 static int recover_on(Ctx& c, int curve, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
                       const uint8_t* recid, uint8_t* out_xy, uint8_t* status) {
   int rc = ensure_table(c, curve);
@@ -1386,29 +1423,54 @@ static int recover_on(Ctx& c, int curve, size_t n, const uint8_t* e, const uint8
   if ((rc = grow(&c.d_ws, &c.d_ws_cap, W.total))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
   uint8_t *d_e = c.d_in, *d_r = d_e + len * n, *d_s = d_r + len * n, *d_out = d_s + len * n, *d_id = d_out + 2 * len * n;
-  u32 *ws = (u32*)(c.d_ws + W.ws), *qtab = (u32*)(c.d_ws + W.qtab);
   return run_single(c, {{d_e, e, len * n}, {d_r, r, len * n}, {d_s, s, len * n}, {d_id, recid, n}},
     [&](Launch& L) {
-      return with_curve(curve, [&](auto cv) {
-        typedef decltype(cv) T;
-        if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;     // eb200_ecdsa_recover_batch refuses it first
-        else {
-          if constexpr (is_k256<T>) {
-            L(k256_prep_recover_kernel, batch_blocks(n, PREP_BATCH), 128, n, d_e, d_r, d_s, ws, (u32*)(c.d_ws + W.scratch));
-            CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
-            L(k256_recover_kernel, (unsigned)((n + EB_VERIFY_BLOCK - 1) / EB_VERIFY_BLOCK), EB_VERIFY_BLOCK, n, d_r, d_id, ws,
-              c.gtab[curve], qtab, d_out, c.d_status);
-          } else {
-            L(sw_prep_recover_kernel<typename T::C>, blocks128(n), 128, n, d_e, d_r, d_s, ws);
-            CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
-            L(sw_recover_kernel<typename T::C>, blocks128(n), 128, n, d_r, d_id, ws, c.gtab[curve], qtab, d_out, c.d_status);
-          }
-          CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
-          return EB200_OK;
-        }
-      });
+      return recover_launches(c, curve, n, d_e, d_r, d_s, d_id, c.d_ws, d_out, c.d_status, L, c.ev[EV_MAIN_BEGIN],
+                              c.ev[EV_MAIN_END]);
     },
     {{out_xy, d_out, 2 * len * n}, {status, c.d_status, n}}, {}, false);
+}
+
+// The launches of one mul / mulAdd / derive block whose inputs are on the device (dk1 == NULL: no base-point term;
+// d_pts == NULL: k2 G): the main kernel between ev0 and ev1, with the scalar prep in front of it and the replay (derive:
+// the status map) behind it for an arbitrary point.  Writes x || y to d_out also for derive.  base: ws_layout(curve,
+// n).total bytes of workspace, of which the scalar prep's digit words and the per-item tables are used.
+static int mul_add_launches(Ctx& c, int curve, size_t n, const uint8_t* dk1, const uint8_t* d_k2, const uint8_t* d_pts,
+                            uint8_t* base, uint8_t* d_out, uint8_t* d_status, bool derive, Launch& L, cudaEvent_t ev0,
+                            cudaEvent_t ev1) {
+  const WsLayout W = ws_layout(curve, n);
+  u32 *ws = (u32*)(base + W.ws), *qtab = (u32*)(base + W.qtab);
+  const unsigned nb = blocks128(n);
+  return with_curve(curve, [&](auto cv) {
+    typedef decltype(cv) T;
+    const u32* gt = c.gtab[curve];
+    if constexpr (is_ed25519<T>) {
+      CK(cudaEventRecord(ev0, L.st));
+      L(ed_ec_mul_add_kernel, nb, 128, n, dk1, d_k2, d_pts, derive ? 1u : 0u, gt, qtab, d_out, d_status);
+      CK(cudaEventRecord(ev1, L.st));
+    } else if (!d_pts) {
+      CK(cudaEventRecord(ev0, L.st));
+      if constexpr (is_k256<T>) L(k256_mul_g_kernel, nb, 128, n, d_k2, gt, d_out, d_status);
+      else L(sw_mul_g_kernel<typename T::C>, nb, 128, n, d_k2, gt, d_out, d_status);
+      CK(cudaEventRecord(ev1, L.st));
+    } else {
+      if constexpr (is_k256<T>) {
+        L(k256_prep_scalars_kernel, nb, 128, n, dk1, d_k2, ws);
+        CK(cudaEventRecord(ev0, L.st));
+        L(k256_mul_add_kernel, (unsigned)((n + EB_VERIFY_BLOCK - 1) / EB_VERIFY_BLOCK), EB_VERIFY_BLOCK, n, d_pts, ws, gt,
+          qtab, d_out, d_status);
+      } else {
+        L(sw_prep_scalars_kernel<typename T::C>, nb, 128, n, dk1, d_k2, ws);
+        CK(cudaEventRecord(ev0, L.st));
+        L(sw_mul_add_kernel<typename T::C>, nb, 128, n, d_pts, ws, gt, qtab, d_out, d_status);
+      }
+      CK(cudaEventRecord(ev1, L.st));
+      if (derive) L(status_map_kernel, nb, 128, n, d_status, (uint8_t)ST_NEEDS_HOST, (uint8_t)ST_THROW_NOT_VALIDATED);
+      else if constexpr (is_k256<T>) L(k256_mul_add_replay_kernel, nb, 128, n, dk1, d_k2, d_pts, c.replay_tab, d_out, d_status);
+      else L(sw_mul_add_replay_kernel<typename T::C>, nb, 128, n, dk1, d_k2, d_pts, c.sw_replay_tab[curve], d_out, d_status);
+    }
+    return EB200_OK;
+  });
 }
 
 // ---- Point.mul / Point.mulAdd batches ---------------------------------------------------------------
@@ -1425,41 +1487,10 @@ static int mul_add_on(Ctx& c, int curve, size_t n, const uint8_t* k1, const uint
   if ((rc = grow(&c.d_ws, &c.d_ws_cap, W.total))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
   uint8_t *d_k1 = c.d_in, *d_k2 = d_k1 + len * n, *d_pts = d_k2 + len * n, *d_out = d_pts + 2 * len * n;
-  const uint8_t* dk1 = k1 ? d_k1 : nullptr;
-  u32 *ws = (u32*)(c.d_ws + W.ws), *qtab = (u32*)(c.d_ws + W.qtab);
-  const unsigned nb = blocks128(n);
   return run_single(c, {{d_k1, k1, k1 ? len * n : 0}, {d_k2, k2, len * n}, {d_pts, pts, pts ? 2 * len * n : 0}},
     [&](Launch& L) {
-      return with_curve(curve, [&](auto cv) {
-        typedef decltype(cv) T;
-        const u32* gt = c.gtab[curve];
-        if constexpr (is_ed25519<T>) {
-          CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
-          L(ed_ec_mul_add_kernel, nb, 128, n, dk1, d_k2, pts ? d_pts : nullptr, derive ? 1u : 0u, gt, qtab, d_out, c.d_status);
-          CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
-        } else if (!pts) {
-          CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
-          if constexpr (is_k256<T>) L(k256_mul_g_kernel, nb, 128, n, d_k2, gt, d_out, c.d_status);
-          else L(sw_mul_g_kernel<typename T::C>, nb, 128, n, d_k2, gt, d_out, c.d_status);
-          CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
-        } else {
-          if constexpr (is_k256<T>) {
-            L(k256_prep_scalars_kernel, nb, 128, n, dk1, d_k2, ws);
-            CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
-            L(k256_mul_add_kernel, (unsigned)((n + EB_VERIFY_BLOCK - 1) / EB_VERIFY_BLOCK), EB_VERIFY_BLOCK, n, d_pts, ws, gt,
-              qtab, d_out, c.d_status);
-          } else {
-            L(sw_prep_scalars_kernel<typename T::C>, nb, 128, n, dk1, d_k2, ws);
-            CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
-            L(sw_mul_add_kernel<typename T::C>, nb, 128, n, d_pts, ws, gt, qtab, d_out, c.d_status);
-          }
-          CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
-          if (derive) L(status_map_kernel, nb, 128, n, c.d_status, (uint8_t)ST_NEEDS_HOST, (uint8_t)ST_THROW_NOT_VALIDATED);
-          else if constexpr (is_k256<T>) L(k256_mul_add_replay_kernel, nb, 128, n, dk1, d_k2, d_pts, c.replay_tab, d_out, c.d_status);
-          else L(sw_mul_add_replay_kernel<typename T::C>, nb, 128, n, dk1, d_k2, d_pts, c.sw_replay_tab[curve], d_out, c.d_status);
-        }
-        return EB200_OK;
-      });
+      return mul_add_launches(c, curve, n, k1 ? d_k1 : nullptr, d_k2, pts ? d_pts : nullptr, c.d_ws, d_out, c.d_status, derive,
+                              L, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
     },
     // derive: x only; its scalars are private keys, which do not stay in the shared staging buffer
     {{out_xy, d_out, derive ? len : 2 * len * n, derive ? n : 1, 2 * len}, {status, c.d_status, n}},
@@ -1480,57 +1511,105 @@ static int mul_add_common(int curve, size_t n, const uint8_t* k1, const uint8_t*
 }
 
 // ---- ECDSA sign (RFC 6979 nonces on the GPU) ---------------------------------------------------------
-// mode: kgiven != NULL -> the caller's nonces, one attempt (items the reference would `continue` on come back as
-// EB200_ST_RETRY); pers != NULL -> the literal loop on the byte-stream DRBG; neither -> RFC 6979 fast pipeline.
+// Workspace of one sign block of n items: the nonce kernel's X, Y, Z and k words | the finish kernel's inversion scratch.
+struct SignWs { size_t scr, total; };
+static SignWs sign_ws(int curve, size_t n) {
+  const size_t limbs = fe_len(curve) / 4;
+  SignWs W;
+  W.scr = align256(4 * limbs * 4 * n);                                // X, Y, Z, k
+  W.total = W.scr + 2 * limbs * 4 * n;
+  return W;
+}
+
+// The launches of one sign block whose inputs are on the device.  mode: kg != NULL -> the caller's nonces, one attempt
+// (items the reference would `continue` on come back as EB200_ST_RETRY); pp != NULL -> the literal loop on the
+// byte-stream DRBG (np bytes of pers; np = 0: none read); neither -> RFC 6979 fast pipeline.  The first kernel (the
+// nonce kernel, or the whole loop) runs between ev0 and ev1.  base: sign_ws(curve, n).total bytes of workspace, which
+// then holds nonces and k G.
+static int sign_launches(Ctx& c, int curve, size_t n, const uint8_t* d_e, const uint8_t* d_k, const uint8_t* kg,
+                         const uint8_t* pp, size_t np, u32 canonical, uint8_t* base, uint8_t* d_r, uint8_t* d_s, uint8_t* d_id,
+                         uint8_t* d_status, Launch& L, cudaEvent_t ev0, cudaEvent_t ev1) {
+  u32 *d_sws = (u32*)base, *d_scr = (u32*)(base + sign_ws(curve, n).scr);
+  const unsigned nb = blocks128(n);
+  return with_curve(curve, [&](auto cv) {
+    typedef decltype(cv) T;
+    const u32* gt = c.gtab[curve];
+    CK(cudaEventRecord(ev0, L.st));
+    if constexpr (is_ed25519<T>) {
+      L(ed_ec_sign_kernel, nb, 128, n, d_e, d_k, kg, pp, (u32)np, canonical, gt, d_r, d_s, d_id, d_status);
+      CK(cudaEventRecord(ev1, L.st));
+    } else if constexpr (is_k256<T>) {
+      if (pp) {
+        L(k256_sign_pers_kernel, nb, 128, n, d_e, d_k, pp, (u32)np, canonical, gt, d_r, d_s, d_id, d_status);
+        CK(cudaEventRecord(ev1, L.st));
+      } else {
+        L(k256_sign_nonce_kernel, nb, 128, n, d_e, d_k, gt, d_sws, d_status, kg);
+        CK(cudaEventRecord(ev1, L.st));
+        L(k256_sign_finish_kernel, batch_blocks(n, PREP_BATCH), 128, n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, d_status);
+        if (kg) L(status_map_kernel, nb, 128, n, d_status, (uint8_t)ST_NEEDS_HOST, (uint8_t)EB200_ST_RETRY);
+        else L(k256_sign_slow_kernel, nb, 128, n, d_e, d_k, canonical, gt, d_r, d_s, d_id, d_status);
+      }
+    } else {
+      typedef typename T::SG SG;
+      if (pp) {
+        L(sw_sign_pers_kernel<SG>, nb, 128, n, d_e, d_k, pp, (u32)np, canonical, gt, d_r, d_s, d_id, d_status);
+        CK(cudaEventRecord(ev1, L.st));
+      } else {
+        L(sw_sign_nonce_kernel<SG>, nb, 128, n, d_e, d_k, gt, d_sws, d_status, kg);
+        CK(cudaEventRecord(ev1, L.st));
+        L(sw_sign_finish_kernel<SG>, batch_blocks(n, SG::BATCH), 128, n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, d_status);
+        if (kg) L(status_map_kernel, nb, 128, n, d_status, (uint8_t)ST_NEEDS_HOST, (uint8_t)EB200_ST_RETRY);
+        else L(sw_sign_slow_kernel<SG>, nb, 128, n, d_e, d_k, canonical, gt, d_r, d_s, d_id, d_status);
+      }
+    }
+    return EB200_OK;
+  });
+}
+
 static int sign_on(Ctx& c, int curve, size_t n, const uint8_t* e, const uint8_t* priv, uint32_t flags,
                    uint8_t* out_r, uint8_t* out_s, uint8_t* out_recid, uint8_t* status,
                    const uint8_t* kgiven = nullptr, const uint8_t* pers = nullptr, size_t np = 0) {
   int rc = ensure_table(c, curve);
   if (rc) return rc;
-  const size_t len = curve_len(curve), limbs = fe_len(curve) / 4;
+  const size_t len = curve_len(curve);
   if ((rc = grow(&c.d_in, &c.d_in_cap, n * (5 * len + 1) + align256(np + 1) + 512))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
-  const size_t ws_bytes = align256(4 * limbs * 4 * n);                 // X, Y, Z, k
-  const size_t scr_bytes = 2 * limbs * 4 * n;
-  if ((rc = grow(&c.d_ws, &c.d_ws_cap, ws_bytes + scr_bytes))) return rc;
+  const SignWs W = sign_ws(curve, n);
+  if ((rc = grow(&c.d_ws, &c.d_ws_cap, W.total))) return rc;
   uint8_t *d_e = c.d_in, *d_k = d_e + len * n, *d_r = d_k + len * n, *d_s = d_r + len * n, *d_kg = d_s + len * n, *d_id = d_kg + len * n;
   uint8_t* d_pers = (uint8_t*)(((uintptr_t)(d_id + n) + 255) & ~(uintptr_t)255);
-  u32 *d_sws = (u32*)c.d_ws, *d_scr = (u32*)(c.d_ws + ws_bytes);
   const u32 canonical = flags & EB200_SIGN_CANONICAL;
   const uint8_t* kg = kgiven ? d_kg : nullptr;
   const uint8_t* pp = pers ? d_pers : nullptr;
-  const unsigned nb = blocks128(n);
   return run_single(c, {{d_e, e, len * n}, {d_k, priv, len * n}, {d_kg, kgiven, kgiven ? len * n : 0}, {d_pers, pers, pers ? np : 0}},
     [&](Launch& L) {
-      return with_curve(curve, [&](auto cv) {
-        typedef decltype(cv) T;
-        const u32* gt = c.gtab[curve];
-        if constexpr (is_ed25519<T>) {
-          L(ed_ec_sign_kernel, nb, 128, n, d_e, d_k, kg, pp, (u32)np, canonical, gt, d_r, d_s, d_id, c.d_status);
-        } else if constexpr (is_k256<T>) {
-          if (pp) L(k256_sign_pers_kernel, nb, 128, n, d_e, d_k, pp, (u32)np, canonical, gt, d_r, d_s, d_id, c.d_status);
-          else {
-            L(k256_sign_nonce_kernel, nb, 128, n, d_e, d_k, gt, d_sws, c.d_status, kg);
-            L(k256_sign_finish_kernel, batch_blocks(n, PREP_BATCH), 128, n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, c.d_status);
-            if (kg) L(status_map_kernel, nb, 128, n, c.d_status, (uint8_t)ST_NEEDS_HOST, (uint8_t)EB200_ST_RETRY);
-            else L(k256_sign_slow_kernel, nb, 128, n, d_e, d_k, canonical, gt, d_r, d_s, d_id, c.d_status);
-          }
-        } else {
-          typedef typename T::SG SG;
-          if (pp) L(sw_sign_pers_kernel<SG>, nb, 128, n, d_e, d_k, pp, (u32)np, canonical, gt, d_r, d_s, d_id, c.d_status);
-          else {
-            L(sw_sign_nonce_kernel<SG>, nb, 128, n, d_e, d_k, gt, d_sws, c.d_status, kg);
-            L(sw_sign_finish_kernel<SG>, batch_blocks(n, SG::BATCH), 128, n, d_e, d_k, canonical, d_sws, d_scr, d_r, d_s, d_id, c.d_status);
-            if (kg) L(status_map_kernel, nb, 128, n, c.d_status, (uint8_t)ST_NEEDS_HOST, (uint8_t)EB200_ST_RETRY);
-            else L(sw_sign_slow_kernel<SG>, nb, 128, n, d_e, d_k, canonical, gt, d_r, d_s, d_id, c.d_status);
-          }
-        }
-        return EB200_OK;
-      });
+      return sign_launches(c, curve, n, d_e, d_k, kg, pp, np, canonical, c.d_ws, d_r, d_s, d_id, c.d_status, L,
+                           c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
     },
     {{out_r, d_r, len * n}, {out_s, d_s, len * n}, {out_recid, d_id, n}, {status, c.d_status, n}},
     // private keys, nonces k and k*G live in buffers that later calls reuse: wipe them before returning
-    {{d_k, len * n}, {d_kg, kgiven ? len * n : 0}, {c.d_ws, ws_bytes + scr_bytes}}, true);
+    {{d_k, len * n}, {d_kg, kgiven ? len * n : 0}, {c.d_ws, W.total}}, true);
+}
+
+// The launches of one genKeyPair block whose inputs are on the device: the keygen kernel (private keys to d_priv, its
+// verdicts to d_status) between ev0 and ev1, then k G to d_pub with the multiplication's statuses in mul_status.
+static int keygen_launches(Ctx& c, int curve, size_t n, const uint8_t* d_ent, size_t ne, const uint8_t* pp, size_t np,
+                           uint8_t* d_priv, uint8_t* d_pub, uint8_t* d_status, uint8_t* mul_status, Launch& L, cudaEvent_t ev0,
+                           cudaEvent_t ev1) {
+  const unsigned nb = blocks128(n);
+  return with_curve(curve, [&](auto cv) {
+    typedef decltype(cv) T;
+    const u32* gt = c.gtab[curve];
+    CK(cudaEventRecord(ev0, L.st));
+    if constexpr (is_k256<T>) L(k256_keygen_kernel, nb, 128, n, d_ent, (u32)ne, pp, (u32)np, d_priv, d_status);
+    else if constexpr (is_ed25519<T>) L(ed_ec_keygen_kernel, nb, 128, n, d_ent, (u32)ne, pp, (u32)np, d_priv, d_status);
+    else L(sw_keygen_kernel<typename T::SG>, nb, 128, n, d_ent, (u32)ne, pp, (u32)np, d_priv, d_status);
+    CK(cudaEventRecord(ev1, L.st));
+    if constexpr (is_k256<T>) L(k256_mul_g_kernel, nb, 128, n, d_priv, gt, d_pub, mul_status);
+    else if constexpr (is_ed25519<T>) L(ed_ec_mul_add_kernel, nb, 128, n, nullptr, d_priv, nullptr, 0u, gt, nullptr, d_pub, mul_status);
+    else L(sw_mul_g_kernel<typename T::C>, nb, 128, n, d_priv, gt, d_pub, mul_status);
+    return EB200_OK;
+  });
 }
 
 // EC.genKeyPair({entropy, pers}) (ec/index.js:55-79): private keys from HMAC-DRBG(entropy_i, nonce = n, pers), then
@@ -1540,32 +1619,21 @@ static int keygen_on(Ctx& c, int curve, size_t n, const uint8_t* entropy, size_t
   int rc = ensure_table(c, curve);
   if (rc) return rc;
   const size_t len = curve_len(curve);
-  if ((rc = grow(&c.d_in, &c.d_in_cap, align256(n * ne) + align256(np + 1) + n * 3 * len + 512))) return rc;
+  if ((rc = grow(&c.d_in, &c.d_in_cap, align256(n * ne) + align256(np + 1) + n * 3 * len + n + 512))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
   uint8_t* d_ent = c.d_in;
   uint8_t* d_pers = d_ent + align256(n * ne);
   uint8_t* d_priv = d_pers + align256(np + 1);
   uint8_t* d_pub = d_priv + len * n;
-  const unsigned nb = blocks128(n);
+  uint8_t* d_mst = d_pub + 2 * len * n;               // the multiplication's statuses (not returned)
   const uint8_t* pp = pers ? d_pers : nullptr;
   return run_single(c, {{d_ent, entropy, n * ne}, {d_pers, pers, pers ? np : 0}},
     [&](Launch& L) {
-      return with_curve(curve, [&](auto cv) {
-        typedef decltype(cv) T;
-        const u32* gt = c.gtab[curve];
-        if constexpr (is_k256<T>) L(k256_keygen_kernel, nb, 128, n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status);
-        else if constexpr (is_ed25519<T>) L(ed_ec_keygen_kernel, nb, 128, n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status);
-        else L(sw_keygen_kernel<typename T::SG>, nb, 128, n, d_ent, (u32)ne, pp, (u32)np, d_priv, c.d_status);
-        if (L.rc) return L.rc;
-        // the keygen verdicts (the mul below reuses d_status)
-        CK(cudaMemcpyAsync(status, c.d_status, n, cudaMemcpyDeviceToHost, L.st));
-        if constexpr (is_k256<T>) L(k256_mul_g_kernel, nb, 128, n, d_priv, gt, d_pub, c.d_status);
-        else if constexpr (is_ed25519<T>) L(ed_ec_mul_add_kernel, nb, 128, n, nullptr, d_priv, nullptr, 0u, gt, nullptr, d_pub, c.d_status);
-        else L(sw_mul_g_kernel<typename T::C>, nb, 128, n, d_priv, gt, d_pub, c.d_status);
-        return EB200_OK;
-      });
+      return keygen_launches(c, curve, n, d_ent, ne, pp, np, d_priv, d_pub, c.d_status, d_mst, L, c.ev[EV_MAIN_BEGIN],
+                             c.ev[EV_MAIN_END]);
     },
-    {{out_priv, d_priv, len * n}, {out_pub, d_pub, 2 * len * n}}, {{d_ent, n * ne}, {d_priv, len * n}}, true);
+    {{out_priv, d_priv, len * n}, {out_pub, d_pub, 2 * len * n}, {status, c.d_status, n}},
+    {{d_ent, n * ne}, {d_priv, len * n}}, true);
 }
 
 extern "C" {
@@ -1672,6 +1740,26 @@ int eb200_eddsa_verify_batch_dev(size_t n, const uint8_t* d_R, const uint8_t* d_
 }
 }  // extern "C"
 
+// The launches of one EdDSA verify block whose inputs are on the device.  msg_off != NULL: h = SHA512(R || A || M) mod n
+// into dh first (msg_off: n + 1 offsets relative to msgs), by the screened hash (keyset_forms.cu) when verdict != NULL;
+// then the verify kernel between ev0 and ev1.  atab: eb200_eddsa_verify_workspace_bytes(n) bytes of workspace.
+static int eddsa_verify_launches(Ctx& c, size_t n, const uint8_t* dR, const uint8_t* dS, const uint8_t* dA, uint8_t* dh,
+                                 const uint8_t* msgs, const u64* msg_off, const uint8_t* verdict, u32* atab, uint8_t* d_status,
+                                 Launch& L, cudaEvent_t ev0, cudaEvent_t ev1) {
+  const unsigned nb = blocks128(n);
+  if (msg_off && verdict) {
+    if (L.rc) return L.rc;
+    cudaError_t err = keyset_ed_hash_screened_launch(n, verdict, dR, dA, msgs, msg_off, dh, L.st, &L.count);
+    if (err != cudaSuccess) return cuda_fail(err, "keyset_ed_hash_screened_launch");
+  } else if (msg_off) {
+    L(ed25519_hash_kernel, nb, 128, n, dR, dA, msgs, msg_off, dh);
+  }
+  CK(cudaEventRecord(ev0, L.st));
+  L(ed25519_verify_kernel, nb, 128, n, dR, dS, dA, (const uint8_t*)dh, c.gtab[EB200_CURVE_ED25519], atab, d_status);
+  CK(cudaEventRecord(ev1, L.st));
+  return L.rc;
+}
+
 // h == NULL: raw messages (msgs + offsets; msg_off points at this block's first offset, offsets absolute), SHA-512 on the GPU
 static int eddsa_on(Ctx& c, size_t n, const uint8_t* R, const uint8_t* S, const uint8_t* A, const uint8_t* h,
                     const uint8_t* msgs, const uint64_t* msg_off, uint8_t* status) {
@@ -1690,7 +1778,6 @@ static int eddsa_on(Ctx& c, size_t n, const uint8_t* R, const uint8_t* S, const 
   uint8_t *dR = c.d_in, *dS = dR + 32 * n, *dA = dS + 32 * n, *dh = dA + 32 * n;
   uint64_t* doff = (uint64_t*)(c.d_in + base);
   uint8_t* dm = c.d_in + base + align256(off_bytes);
-  const u32* gt = c.gtab[EB200_CURVE_ED25519];
   return run_chunked(c, P,
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {dR + 32 * lo, R + 32 * lo, 32 * m};
@@ -1702,18 +1789,33 @@ static int eddsa_on(Ctx& c, size_t n, const uint8_t* R, const uint8_t* S, const 
       return 5;
     },
     [&](size_t lo, size_t m, Launch& L, int slot, int k) {
-      const unsigned nb = blocks128(m);
-      if (!h) L(ed25519_hash_kernel, nb, 128, m, dR + 32 * lo, dA + 32 * lo, dm - msg_off[0], doff + lo, dh + 32 * lo);
-      CK(cudaEventRecord(c.ev_k0[k], L.st));
-      L(ed25519_verify_kernel, nb, 128, m, dR + 32 * lo, dS + 32 * lo, dA + 32 * lo, dh + 32 * lo, gt,
-        (u32*)(c.d_ws + (size_t)slot * ws_slot), c.d_status + lo);
-      CK(cudaEventRecord(c.ev_k1[k], L.st));
-      return EB200_OK;
+      return eddsa_verify_launches(c, m, dR + 32 * lo, dS + 32 * lo, dA + 32 * lo, dh + 32 * lo, h ? nullptr : dm - msg_off[0],
+                                   h ? nullptr : doff + lo, nullptr, (u32*)(c.d_ws + (size_t)slot * ws_slot), c.d_status + lo, L,
+                                   c.ev_k0[k], c.ev_k1[k]);
     },
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {status + lo, c.d_status + lo, m};
       return 1;
     });
+}
+
+// The sign kernel of one EDDSA.sign block whose inputs are on the device (msg_off: n + 1 offsets relative to msgs), or its
+// screened form (unkeyed_forms.cu) when verdict != NULL, between ev0 and ev1.  pub may be NULL.
+static int eddsa_sign_launches(Ctx& c, size_t n, const uint8_t* dsec, const uint8_t* msgs, const u64* msg_off,
+                               const uint8_t* verdict, uint8_t* dsig, uint8_t* dpub, uint8_t* d_status, Launch& L,
+                               cudaEvent_t ev0, cudaEvent_t ev1) {
+  const u32* gt = c.gtab[EB200_CURVE_ED25519];
+  CK(cudaEventRecord(ev0, L.st));
+  if (verdict) {
+    if (L.rc) return L.rc;
+    cudaError_t err = unkeyed_ed25519_sign_screened_launch(n, verdict, dsec, msgs, msg_off, gt, dsig, dpub, d_status, L.st,
+                                                           &L.count);
+    if (err != cudaSuccess) return cuda_fail(err, "unkeyed_ed25519_sign_screened_launch");
+  } else {
+    L(ed25519_sign_kernel, blocks128(n), 128, n, dsec, msgs, msg_off, gt, dsig, dpub, d_status);
+  }
+  CK(cudaEventRecord(ev1, L.st));
+  return L.rc;
 }
 
 // EDDSA.sign batch: secrets n x 32, raw messages (offsets absolute, msg_off points at this block's first one)
@@ -1731,11 +1833,21 @@ static int eddsa_sign_on(Ctx& c, size_t n, const uint8_t* secrets, const uint8_t
   uint8_t* dm = c.d_in + base + align256(off_bytes);
   return run_single(c, {{dsec, secrets, 32 * n}, {doff, msg_off, off_bytes}, {dm, msgs + msg_off[0], mbytes}},
     [&](Launch& L) {
-      L(ed25519_sign_kernel, blocks128(n), 128, n, dsec, dm - msg_off[0], doff, c.gtab[EB200_CURVE_ED25519], dsig, dpub, c.d_status);
-      return EB200_OK;
+      return eddsa_sign_launches(c, n, dsec, dm - msg_off[0], doff, nullptr, dsig, dpub, c.d_status, L, c.ev[EV_MAIN_BEGIN],
+                                 c.ev[EV_MAIN_END]);
     },
     {{sig, dsig, 64 * n}, {pub, dpub, 32 * n}, {status, c.d_status, n}},
     {{dsec, 32 * n}}, true);             // secrets do not stay in the shared buffer
+}
+
+// The curve25519 kernel of one block whose inputs are on the device, between ev0 and ev1: the ladder with MontCurve.validate
+// (KeyPair.derive) or without it (Point.mul).
+static int x25519_launches(size_t n, const uint8_t* dk, const uint8_t* dx, uint8_t* dout, uint8_t* d_status, bool validate,
+                           Launch& L, cudaEvent_t ev0, cudaEvent_t ev1) {
+  CK(cudaEventRecord(ev0, L.st));
+  L(validate ? x25519_derive_kernel : x25519_mul_kernel, blocks128(n), 128, n, dk, dx, dout, d_status);
+  CK(cudaEventRecord(ev1, L.st));
+  return L.rc;
 }
 
 static int x25519_on(Ctx& c, size_t n, const uint8_t* priv, const uint8_t* pubx, uint8_t* out, uint8_t* status, bool validate) {
@@ -1751,10 +1863,9 @@ static int x25519_on(Ctx& c, size_t n, const uint8_t* priv, const uint8_t* pubx,
       return 2;
     },
     [&](size_t lo, size_t m, Launch& L, int, int k) {
-      CK(cudaEventRecord(c.ev_k0[k], L.st));
-      L(validate ? x25519_derive_kernel : x25519_mul_kernel, blocks128(m), 128, m, dk + 32 * lo, dx + 32 * lo, dout + 32 * lo,
-        c.d_status + lo);
-      CK(cudaEventRecord(c.ev_k1[k], L.st));
+      int rc2 = x25519_launches(m, dk + 32 * lo, dx + 32 * lo, dout + 32 * lo, c.d_status + lo, validate, L, c.ev_k0[k],
+                                c.ev_k1[k]);
+      if (rc2) return rc2;
       CK(cudaMemsetAsync(dk + 32 * lo, 0, 32 * m, L.st));   // private scalars do not stay in the shared buffer
       return EB200_OK;
     },
@@ -1811,10 +1922,7 @@ int eb200_x25519_derive_batch_dev(size_t n, const uint8_t* d_priv, const uint8_t
   if (n == 0) return eb200_device_count() ? EB200_OK : EB200_ERR_NOT_INIT;
   if (!d_priv || !d_pubx || !d_out || !d_status) return EB200_ERR_ARG;
   return run_dev(d_status, 0, stream, [&](Ctx& c, Launch& L) {
-    CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
-    L(x25519_derive_kernel, blocks128(n), 128, n, d_priv, d_pubx, d_out, d_status);
-    CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
-    return EB200_OK;
+    return x25519_launches(n, d_priv, d_pubx, d_out, d_status, true, L, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
   });
 }
 
@@ -2031,6 +2139,17 @@ int eb200_selftest_gtab(int curve, uint32_t* out, size_t n_words) {
 
 // ---- EC.getKeyRecoveryParam ----------------------------------------------------------------------------------------
 // The kernels are in recovery_param.cu (see there why); this side stages the buffers and runs them like recover_on.
+// The launches of one block whose inputs are on the device; base: ws_layout(curve, n).total bytes of workspace.
+static int recovery_param_launches(Ctx& c, int curve, size_t n, const uint8_t* d_e, const uint8_t* d_r, const uint8_t* d_s,
+                                   const uint8_t* d_q, uint8_t* d_id, uint8_t* d_status, uint8_t* base, Launch& L,
+                                   cudaEvent_t ev0, cudaEvent_t ev1) {
+  const WsLayout W = ws_layout(curve, n);
+  const RecoveryParamArgs a{d_e, d_r, d_s, d_q, d_id, d_status, c.gtab[curve], (u32*)(base + W.ws), (u32*)(base + W.scratch),
+                            (u32*)(base + W.qtab)};
+  cudaError_t err = recovery_param_launch(curve, n, a, L.st, ev0, ev1, &L.count);
+  return err == cudaSuccess ? EB200_OK : cuda_fail(err, "recovery_param_launch");
+}
+
 static int recovery_param_on(Ctx& c, int curve, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
                              const uint8_t* q_xy, uint8_t* out_recid, uint8_t* status) {
   int rc = ensure_table(c, curve);
@@ -2041,12 +2160,10 @@ static int recovery_param_on(Ctx& c, int curve, size_t n, const uint8_t* e, cons
   if ((rc = grow(&c.d_ws, &c.d_ws_cap, W.total))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
   uint8_t *d_e = c.d_in, *d_r = d_e + len * n, *d_s = d_r + len * n, *d_q = d_s + len * n, *d_id = d_q + 2 * len * n;
-  u32 *ws = (u32*)(c.d_ws + W.ws), *qtab = (u32*)(c.d_ws + W.qtab);
   return run_single(c, {{d_e, e, len * n}, {d_r, r, len * n}, {d_s, s, len * n}, {d_q, q_xy, 2 * len * n}},
     [&](Launch& L) {
-      const RecoveryParamArgs a{d_e, d_r, d_s, d_q, d_id, c.d_status, c.gtab[curve], ws, (u32*)(c.d_ws + W.scratch), qtab};
-      cudaError_t err = recovery_param_launch(curve, n, a, L.st, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END], &L.count);
-      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "recovery_param_launch");
+      return recovery_param_launches(c, curve, n, d_e, d_r, d_s, d_q, d_id, c.d_status, c.d_ws, L, c.ev[EV_MAIN_BEGIN],
+                                     c.ev[EV_MAIN_END]);
     },
     {{out_recid, d_id, n}, {status, c.d_status, n}}, {}, false);     // nothing secret: no wipe
 }
@@ -3084,6 +3201,240 @@ int eb200_x25519_derive_batch_keyed_dev(const eb200_keyset* ks, size_t n, const 
         return cuda_fail(err, "keyset_verdict_merge_out_launch");
       CK(cudaMemsetAsync(body, 0, keyed_dev_body_bytes(ks, n), L.st));   // the scalars and the per-item results
       return EB200_OK;
+    });
+}
+
+}  // extern "C"
+
+// ---- device-pointer forms of the unkeyed calls ---------------------------------------------------------------------------
+// Each runs its host form's launch sequence (the *_launches functions above) on the caller's stream through run_dev, with
+// the workspace regions as dev_ws places them, and the calls with variable-length ranges put a range screen in front and
+// a verdict merge behind it.
+namespace {
+// The workspace of the unkeyed device-pointer calls on `curve`, n items.  Every call places its regions from the start:
+//   verify, recover, getKeyRecoveryParam, mul / mulAdd / derive, ed25519 verify: ws_layout(curve, n) (on ed25519 its
+//     first region is the verify kernel's per-item tables);
+//   then [verdict, rows): per-item bytes -- range verdicts (DER verify, ed25519 messages, EdDSA sign) or keygen's
+//     multiplication statuses;
+//   then [rows, total): 2 len bytes per item -- decoded r, s (DER verify), x || y (derive), k G (keygen without
+//     d_out_pub_xy), h (ed25519 messages, 32 bytes per item);
+//   sign alone places sign_ws(curve, n) from the start.
+struct DevWs { size_t verdict, rows, total; };
+DevWs dev_ws(int curve, size_t n) {
+  DevWs D;
+  D.verdict = ws_layout(curve, n).total;
+  D.rows = D.verdict + align256(n);
+  D.total = D.rows + align256(2 * curve_len(curve) * n);
+  const size_t sign = sign_ws(curve, n).total;
+  if (sign > D.total) D.total = sign;
+  return D;
+}
+
+// n = 0 and the argument checks of an unkeyed device-pointer call, after its curve check: DEV_GO to go on, else what to
+// return -- EB200_OK (n = 0 with a device) or EB200_ERR_NOT_INIT (without), EB200_ERR_ARG for a refused argument.
+constexpr int DEV_GO = 1;
+int dev_checks(size_t n, bool args_ok) {
+  if (n == 0) return eb200_device_count() ? EB200_OK : EB200_ERR_NOT_INIT;
+  return args_ok ? DEV_GO : EB200_ERR_ARG;
+}
+
+int sign_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_priv, const uint8_t* d_k, const uint8_t* d_pers,
+             size_t pers_len, bool pers, uint32_t flags, uint8_t* d_out_r, uint8_t* d_out_s, uint8_t* d_out_recid,
+             uint8_t* d_status, void* d_workspace, void* stream, bool need_k) {
+  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
+  int rc = dev_checks(n, d_e && d_priv && (d_k || !need_k) && d_out_r && d_out_s && d_out_recid && d_status && d_workspace &&
+                             (!pers || ((d_pers || !pers_len) && pers_len <= (1u << 20))));
+  if (rc != DEV_GO) return rc;
+  return run_dev(d_status, curve, stream, [&](Ctx& c, Launch& L) {
+    // pers with pers_len = 0: the kernel reads no byte of it, but a non-NULL pointer selects the pers loop
+    const uint8_t* pp = !pers ? nullptr : pers_len ? d_pers : d_status;
+    uint8_t* base = (uint8_t*)d_workspace;
+    int rc2 = sign_launches(c, curve, n, d_e, d_priv, need_k ? d_k : nullptr, pp, pers ? pers_len : 0,
+                            flags & EB200_SIGN_CANONICAL, base, d_out_r, d_out_s, d_out_recid, d_status, L,
+                            c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
+    if (rc2) return rc2;
+    CK(cudaMemsetAsync(base, 0, sign_ws(curve, n).total, L.st));     // nonces, k G, the finish kernel's scratch
+    return EB200_OK;
+  });
+}
+
+int mul_add_dev(int curve, size_t n, const uint8_t* d_k1, const uint8_t* d_k2, const uint8_t* d_pts, uint8_t* d_out,
+                uint8_t* d_status, void* d_workspace, void* stream, bool args_ok, bool derive) {
+  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
+  int rc = dev_checks(n, args_ok && d_k2 && d_out && d_status && d_workspace);
+  if (rc != DEV_GO) return rc;
+  return run_dev(d_status, curve, stream, [&](Ctx& c, Launch& L) {
+    const size_t len = curve_len(curve);
+    const DevWs D = dev_ws(curve, n);
+    uint8_t* base = (uint8_t*)d_workspace;
+    int rc2 = mul_add_launches(c, curve, n, d_k1, d_k2, d_pts, base, derive ? base + D.rows : d_out, d_status, derive, L,
+                               c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
+    if (rc2 || !derive) return rc2;
+    CK(cudaMemcpy2DAsync(d_out, len, base + D.rows, 2 * len, len, n, cudaMemcpyDeviceToDevice, L.st));   // x of x || y
+    CK(cudaMemsetAsync(base, 0, D.total, L.st));     // the scalars' digit words, the per-item tables, x || y
+    return EB200_OK;
+  });
+}
+
+// The range-screened calls: the range screen into the verdicts at dev_ws's `verdict`, then run(c, L, verdict, base).
+template <class Run>
+int range_screened_dev(int table_curve, size_t n, const uint64_t* d_off, uint64_t len, uint8_t* d_status, void* d_workspace,
+                       void* stream, Run&& run) {
+  return run_dev(d_status, table_curve, stream, [&](Ctx& c, Launch& L) {
+    uint8_t* base = (uint8_t*)d_workspace;
+    uint8_t* verdict = base + dev_ws(table_curve, n).verdict;
+    cudaError_t err = unkeyed_range_screen_launch(n, d_off, len, verdict, L.st, &L.count);
+    if (err != cudaSuccess) return cuda_fail(err, "unkeyed_range_screen_launch");
+    return run(c, L, verdict, base);
+  });
+}
+}  // namespace
+
+extern "C" {
+
+size_t eb200_dev_workspace_bytes(int curve, size_t n) {
+  if (!curve_ok(curve)) return 0;
+  return dev_ws(curve, n).total;
+}
+
+int eb200_ecdsa_sign_batch_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_priv, uint32_t flags, uint8_t* d_out_r,
+                               uint8_t* d_out_s, uint8_t* d_out_recid, uint8_t* d_status, void* d_workspace, void* stream) {
+  return sign_dev(curve, n, d_e, d_priv, nullptr, nullptr, 0, false, flags, d_out_r, d_out_s, d_out_recid, d_status,
+                  d_workspace, stream, false);
+}
+
+int eb200_ecdsa_sign_batch_k_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_priv, const uint8_t* d_k,
+                                 uint32_t flags, uint8_t* d_out_r, uint8_t* d_out_s, uint8_t* d_out_recid, uint8_t* d_status,
+                                 void* d_workspace, void* stream) {
+  return sign_dev(curve, n, d_e, d_priv, d_k, nullptr, 0, false, flags, d_out_r, d_out_s, d_out_recid, d_status, d_workspace,
+                  stream, true);
+}
+
+int eb200_ecdsa_sign_batch_pers_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_priv, const uint8_t* d_pers,
+                                    size_t pers_len, uint32_t flags, uint8_t* d_out_r, uint8_t* d_out_s, uint8_t* d_out_recid,
+                                    uint8_t* d_status, void* d_workspace, void* stream) {
+  return sign_dev(curve, n, d_e, d_priv, nullptr, d_pers, pers_len, true, flags, d_out_r, d_out_s, d_out_recid, d_status,
+                  d_workspace, stream, false);
+}
+
+// workspace: the multiplication's statuses at dev_ws's `verdict`, k G at `rows` when d_out_pub_xy is NULL; both cleared
+int eb200_ec_keygen_batch_dev(int curve, size_t n, const uint8_t* d_entropy, size_t entropy_len, const uint8_t* d_pers,
+                              size_t pers_len, uint8_t* d_out_priv, uint8_t* d_out_pub_xy, uint8_t* d_status, void* d_workspace,
+                              void* stream) {
+  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
+  int rc = dev_checks(n, d_entropy && entropy_len && d_out_priv && d_status && d_workspace && (d_pers || !pers_len) &&
+                             pers_len <= (1u << 20) && entropy_len <= (1u << 16));
+  if (rc != DEV_GO) return rc;
+  return run_dev(d_status, curve, stream, [&](Ctx& c, Launch& L) {
+    const DevWs D = dev_ws(curve, n);
+    uint8_t* base = (uint8_t*)d_workspace;
+    int rc2 = keygen_launches(c, curve, n, d_entropy, entropy_len, pers_len ? d_pers : nullptr, pers_len, d_out_priv,
+                              d_out_pub_xy ? d_out_pub_xy : base + D.rows, d_status, base + D.verdict, L, c.ev[EV_MAIN_BEGIN],
+                              c.ev[EV_MAIN_END]);
+    if (rc2) return rc2;
+    CK(cudaMemsetAsync(base + D.verdict, 0, D.total - D.verdict, L.st));
+    return EB200_OK;
+  });
+}
+
+int eb200_ecdsa_recover_batch_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_r, const uint8_t* d_s,
+                                  const uint8_t* d_recid, uint8_t* d_out_xy, uint8_t* d_status, void* d_workspace, void* stream) {
+  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
+  int rc = dev_checks(n, d_e && d_r && d_s && d_recid && d_out_xy && d_status && d_workspace);
+  if (rc != DEV_GO) return rc;
+  if (curve == EB200_CURVE_ED25519) return EB200_ERR_UNSUPPORTED;      // as eb200_ecdsa_recover_batch
+  return run_dev(d_status, curve, stream, [&](Ctx& c, Launch& L) {
+    return recover_launches(c, curve, n, d_e, d_r, d_s, d_recid, (uint8_t*)d_workspace, d_out_xy, d_status, L,
+                            c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
+  });
+}
+
+int eb200_ecdsa_recovery_param_batch_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_r, const uint8_t* d_s,
+                                         const uint8_t* d_q_xy, uint8_t* d_out_recid, uint8_t* d_status, void* d_workspace,
+                                         void* stream) {
+  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
+  int rc = dev_checks(n, d_e && d_r && d_s && d_q_xy && d_out_recid && d_status && d_workspace);
+  if (rc != DEV_GO) return rc;
+  if (curve == EB200_CURVE_ED25519) return EB200_ERR_UNSUPPORTED;      // as eb200_ecdsa_recovery_param_batch
+  return run_dev(d_status, curve, stream, [&](Ctx& c, Launch& L) {
+    return recovery_param_launches(c, curve, n, d_e, d_r, d_s, d_q_xy, d_out_recid, d_status, (uint8_t*)d_workspace, L,
+                                   c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
+  });
+}
+
+int eb200_scalar_mul_batch_dev(int curve, size_t n, const uint8_t* d_k, const uint8_t* d_points_xy, uint8_t* d_out_xy,
+                               uint8_t* d_status, void* d_workspace, void* stream) {
+  return mul_add_dev(curve, n, nullptr, d_k, d_points_xy, d_out_xy, d_status, d_workspace, stream, true, false);
+}
+
+int eb200_mul_add_batch_dev(int curve, size_t n, const uint8_t* d_k1, const uint8_t* d_k2, const uint8_t* d_p2_xy,
+                            uint8_t* d_out_xy, uint8_t* d_status, void* d_workspace, void* stream) {
+  return mul_add_dev(curve, n, d_k1, d_k2, d_p2_xy, d_out_xy, d_status, d_workspace, stream, d_k1 && d_p2_xy, false);
+}
+
+int eb200_ecdh_derive_batch_dev(int curve, size_t n, const uint8_t* d_priv, const uint8_t* d_pub_xy, uint8_t* d_out_x,
+                                uint8_t* d_status, void* d_workspace, void* stream) {
+  return mul_add_dev(curve, n, nullptr, d_priv, d_pub_xy, d_out_x, d_status, d_workspace, stream, d_pub_xy != nullptr, true);
+}
+
+int eb200_x25519_mul_batch_dev(size_t n, const uint8_t* d_k, const uint8_t* d_px, uint8_t* d_out_x, uint8_t* d_status,
+                               void* stream) {
+  int rc = dev_checks(n, d_k && d_px && d_out_x && d_status);
+  if (rc != DEV_GO) return rc;
+  return run_dev(d_status, 0, stream, [&](Ctx& c, Launch& L) {
+    return x25519_launches(n, d_k, d_px, d_out_x, d_status, false, L, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
+  });
+}
+
+// workspace: launch_verify's (ws_layout), the range verdicts, the decoded r and s
+int eb200_ecdsa_verify_batch_der_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_sigs, uint64_t sigs_len,
+                                     const uint64_t* d_sig_off, const uint8_t* d_pub, uint32_t pub_fmt, uint8_t* d_status,
+                                     void* d_workspace, void* stream) {
+  if (!curve_ok(curve) || !fmt_ok(pub_fmt)) return EB200_ERR_UNSUPPORTED;
+  int rc = dev_checks(n, d_e && (d_sigs || !sigs_len) && d_sig_off && d_pub && d_status && d_workspace);
+  if (rc != DEV_GO) return rc;
+  return range_screened_dev(curve, n, d_sig_off, sigs_len, d_status, d_workspace, stream,
+    [&](Ctx& c, Launch& L, uint8_t* verdict, uint8_t* base) {
+      const size_t len = curve_len(curve);
+      uint8_t* r = base + dev_ws(curve, n).rows;
+      int rc2 = launch_verify(c, curve, n, d_e, r, r + len * n, d_pub, pub_fmt, d_status, base, L, c.ev[EV_MAIN_BEGIN],
+                              c.ev[EV_MAIN_END], d_sigs, (const unsigned long long*)d_sig_off, verdict);
+      if (rc2) return rc2;
+      cudaError_t err = keyset_verdict_merge_launch(n, verdict, d_status, L.st, &L.count);
+      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_verdict_merge_launch");
+    });
+}
+
+// workspace: the verify kernel's tables (ws_layout), the range verdicts, h
+int eb200_eddsa_verify_batch_msgs_dev(size_t n, const uint8_t* d_R, const uint8_t* d_S, const uint8_t* d_A,
+                                      const uint8_t* d_msgs, uint64_t msgs_len, const uint64_t* d_msg_off, uint8_t* d_status,
+                                      void* d_workspace, void* stream) {
+  int rc = dev_checks(n, d_R && d_S && d_A && (d_msgs || !msgs_len) && d_msg_off && d_status && d_workspace);
+  if (rc != DEV_GO) return rc;
+  return range_screened_dev(EB200_CURVE_ED25519, n, d_msg_off, msgs_len, d_status, d_workspace, stream,
+    [&](Ctx& c, Launch& L, uint8_t* verdict, uint8_t* base) {
+      uint8_t* h = base + dev_ws(EB200_CURVE_ED25519, n).rows;
+      int rc2 = eddsa_verify_launches(c, n, d_R, d_S, d_A, h, d_msgs, d_msg_off, verdict, (u32*)base, d_status, L,
+                                      c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
+      if (rc2) return rc2;
+      cudaError_t err = keyset_verdict_merge_launch(n, verdict, d_status, L.st, &L.count);
+      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_verdict_merge_launch");
+    });
+}
+
+// workspace: the range verdicts alone (the sign kernel keeps its secrets in registers and local memory)
+int eb200_eddsa_sign_batch_dev(size_t n, const uint8_t* d_secrets, const uint8_t* d_msgs, uint64_t msgs_len,
+                               const uint64_t* d_msg_off, uint8_t* d_out_sig, uint8_t* d_out_pub, uint8_t* d_status,
+                               void* d_workspace, void* stream) {
+  int rc = dev_checks(n, d_secrets && (d_msgs || !msgs_len) && d_msg_off && d_out_sig && d_status && d_workspace);
+  if (rc != DEV_GO) return rc;
+  return range_screened_dev(EB200_CURVE_ED25519, n, d_msg_off, msgs_len, d_status, d_workspace, stream,
+    [&](Ctx& c, Launch& L, uint8_t* verdict, uint8_t*) {
+      int rc2 = eddsa_sign_launches(c, n, d_secrets, d_msgs, d_msg_off, verdict, d_out_sig, d_out_pub, d_status, L,
+                                    c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
+      if (rc2) return rc2;
+      cudaError_t err = keyset_verdict_merge_out_launch(n, verdict, d_status, d_out_sig, 64, L.st, &L.count);
+      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_verdict_merge_out_launch");
     });
 }
 

@@ -518,6 +518,90 @@ int eb200_eddsa_sign_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uin
 int eb200_x25519_derive_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_priv, const uint32_t* d_key_idx,
                                         uint8_t* d_out_x, uint8_t* d_status, void* d_workspace, void* stream);
 
+/* Device-pointer forms of the unkeyed calls (every compute entry point above except the eb200_curve_* calls), for CUDA
+ * callers whose data is already on the GPU.  Each takes its host form's arguments as DEVICE pointers (d_*), then
+ * d_workspace and a CUDA stream (cudaStream_t cast to void*; NULL = the CUDA default stream), and runs asynchronously on
+ * that stream on the device that owns d_status; the caller synchronises the stream.  The call does not synchronise the
+ * stream or the device, except for the first-use build of a curve's fixed-base table on that device, which
+ * eb200_ecdsa_verify_batch_dev shares.  d_workspace (device memory on that device) must hold
+ * eb200_dev_workspace_bytes(curve, n) bytes, one size for every unkeyed device-pointer call on the curve (those on ed25519
+ * included, and the existing eb200_ecdsa_verify_batch_dev and eb200_eddsa_verify_batch_dev); the call never reads it
+ * before writing it.  The curve25519 calls take no workspace.
+ * Outputs and statuses: for every item whose arguments the host form accepts, byte for byte what the host form writes,
+ * every status included (off-curve points replayed on the short curves, NEEDS_HOST for an off-curve ed25519 point, RETRY,
+ * INFINITY, THROW_SECOND_KEY, THROW_NO_RECOVERY, the cold path for s = 0 mod n).
+ * The calls with variable-length ranges take `len` bytes at d_sigs / d_msgs (NULL only when len = 0) and n + 1 offsets
+ * into them.  A host form refuses a decreasing offset with EB200_ERR_ARG; a device call cannot without synchronising the
+ * stream, so an item with off[i + 1] < off[i] or off[i + 1] > len gets EB200_ST_BAD_ITEM, its outputs are zeroed and its
+ * range is never read.  For DER verify BAD_ITEM takes precedence over a key's throw (the host form refuses the whole
+ * call).
+ * Returned before any launch, in this order: EB200_ERR_UNSUPPORTED for an unknown curve or pub_fmt; for n = 0, EB200_OK
+ * when a device is initialised, else EB200_ERR_NOT_INIT; EB200_ERR_ARG for a NULL pointer (other than those stated) or a
+ * pers_len / entropy_len the host form refuses; EB200_ERR_NOT_INIT for d_status on a device eb200_init has not set up.
+ * recover and getKeyRecoveryParam on ed25519 return EB200_ERR_UNSUPPORTED after the pointer checks, as their host forms.
+ * Secrets: sign (all three forms), keygen, ECDH derive and EdDSA sign clear, on the stream before their work ends, every
+ * workspace region that held scalar-derived data -- sign: the nonces, k G and the finish kernel's inversion scratch;
+ * keygen: k G (when d_out_pub_xy is NULL) and the multiplication's statuses; derive: the scalars' digit words, the
+ * per-item tables and the results x || y; EdDSA sign keeps nothing secret in the workspace (the range verdicts only).
+ * The caller's own buffers are the caller's.
+ * eb200_last_timing (after the caller has synchronised the stream): kernel_ms = the whole call, main_kernel_ms = the
+ * dominant kernel (named per call below), launches as stated per call. */
+size_t eb200_dev_workspace_bytes(int curve, size_t n);   /* 0 for an unknown curve and for curve25519; at least
+                                                            eb200_ecdsa_verify_workspace_bytes(curve, n), and on ed25519
+                                                            eb200_eddsa_verify_workspace_bytes(n) */
+/* Sign: main = the nonce kernel (the whole loop with pers, and on ed25519).  launches = 3 (nonce, finish, then the slow
+ * path, or for _k the RETRY map), 1 with pers or on ed25519.  With _k, an item whose status is RETRY gets no r, s or
+ * recid: those output bytes are left as they were (the host form returns its staging buffer's bytes there). */
+int eb200_ecdsa_sign_batch_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_priv, uint32_t flags, uint8_t* d_out_r,
+                               uint8_t* d_out_s, uint8_t* d_out_recid, uint8_t* d_status, void* d_workspace, void* stream);
+int eb200_ecdsa_sign_batch_k_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_priv, const uint8_t* d_k,
+                                 uint32_t flags, uint8_t* d_out_r, uint8_t* d_out_s, uint8_t* d_out_recid, uint8_t* d_status,
+                                 void* d_workspace, void* stream);
+int eb200_ecdsa_sign_batch_pers_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_priv, const uint8_t* d_pers,
+                                    size_t pers_len, uint32_t flags, uint8_t* d_out_r, uint8_t* d_out_s, uint8_t* d_out_recid,
+                                    uint8_t* d_status, void* d_workspace, void* stream);
+/* Keygen: d_status gets the keygen verdicts; d_out_pub_xy may be NULL.  main = the keygen kernel; launches = 2 (keygen,
+ * k G). */
+int eb200_ec_keygen_batch_dev(int curve, size_t n, const uint8_t* d_entropy, size_t entropy_len, const uint8_t* d_pers,
+                              size_t pers_len, uint8_t* d_out_priv, uint8_t* d_out_pub_xy, uint8_t* d_status, void* d_workspace,
+                              void* stream);
+/* recoverPubKey: main = the recovery kernel; launches = 2 (prep, recovery).  getKeyRecoveryParam: main = its main
+ * kernel; launches = 3 (prep, main, cold kernel for s = 0 mod n). */
+int eb200_ecdsa_recover_batch_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_r, const uint8_t* d_s,
+                                  const uint8_t* d_recid, uint8_t* d_out_xy, uint8_t* d_status, void* d_workspace, void* stream);
+int eb200_ecdsa_recovery_param_batch_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_r, const uint8_t* d_s,
+                                         const uint8_t* d_q_xy, uint8_t* d_out_recid, uint8_t* d_status, void* d_workspace,
+                                         void* stream);
+/* Point.mul (d_points_xy NULL = the base point), mulAdd, ECDH derive: main = the multiplication kernel; launches = 3
+ * (scalar prep, main, replay; derive: the status map), 1 for G.mul and on ed25519.  derive writes x to d_out_x with a
+ * strided device-to-device copy of the x || y it keeps in the workspace. */
+int eb200_scalar_mul_batch_dev(int curve, size_t n, const uint8_t* d_k, const uint8_t* d_points_xy, uint8_t* d_out_xy,
+                               uint8_t* d_status, void* d_workspace, void* stream);
+int eb200_mul_add_batch_dev(int curve, size_t n, const uint8_t* d_k1, const uint8_t* d_k2, const uint8_t* d_p2_xy,
+                            uint8_t* d_out_xy, uint8_t* d_status, void* d_workspace, void* stream);
+int eb200_ecdh_derive_batch_dev(int curve, size_t n, const uint8_t* d_priv, const uint8_t* d_pub_xy, uint8_t* d_out_x,
+                                uint8_t* d_status, void* d_workspace, void* stream);
+/* curve25519 Point.mul: no workspace, as eb200_x25519_derive_batch_dev.  main = the ladder; launches = 1. */
+int eb200_x25519_mul_batch_dev(size_t n, const uint8_t* d_k, const uint8_t* d_px, uint8_t* d_out_x, uint8_t* d_status,
+                               void* stream);
+/* Verify from DER: d_sig_off holds n + 1 offsets into the sigs_len bytes at d_sigs.  main = the verify kernel; launches =
+ * the host form's (SEC1 decode when pub_fmt is not XY, DER decode, prep, verify, replay; on ed25519 no prep and no
+ * replay) + 2 (range screen, merge); the DER decode is a screened form of the host form's, which reads no byte of a
+ * screened item. */
+int eb200_ecdsa_verify_batch_der_dev(int curve, size_t n, const uint8_t* d_e, const uint8_t* d_sigs, uint64_t sigs_len,
+                                     const uint64_t* d_sig_off, const uint8_t* d_pub, uint32_t pub_fmt, uint8_t* d_status,
+                                     void* d_workspace, void* stream);
+/* EdDSA verify from raw messages (workspace: eb200_dev_workspace_bytes(EB200_CURVE_ED25519, n)).  main = the verify
+ * kernel; launches = 4 (range screen, screened hash, verify, merge). */
+int eb200_eddsa_verify_batch_msgs_dev(size_t n, const uint8_t* d_R, const uint8_t* d_S, const uint8_t* d_A,
+                                      const uint8_t* d_msgs, uint64_t msgs_len, const uint64_t* d_msg_off, uint8_t* d_status,
+                                      void* d_workspace, void* stream);
+/* EdDSA sign (workspace as above); d_out_pub may be NULL.  main = the sign kernel; launches = 3 (range screen, screened
+ * sign, merge). */
+int eb200_eddsa_sign_batch_dev(size_t n, const uint8_t* d_secrets, const uint8_t* d_msgs, uint64_t msgs_len,
+                               const uint64_t* d_msg_off, uint8_t* d_out_sig, uint8_t* d_out_pub, uint8_t* d_status,
+                               void* d_workspace, void* stream);
+
 /* Self-test hooks used by the parity tests (device arithmetic vs the oracle).
  * a, b, out: n elements of L little-endian 32-bit limbs each (host pointers); L = 8, except p192 6, p384 12 and
  * p521 18.  An op the curve does not know returns a (short curves) or 0 (secp256k1, ed25519 / curve25519).
