@@ -12,12 +12,12 @@
 // GPU-first algorithm (same outputs, different schedule):
 //   kernel 1 (prep): Montgomery-trick batch inversion of s over 16-32 items/thread,
 //     u1 = e/s, u2 = r/s, GLV split of u2 into odd (k1,k2), regular recoding.
-//   kernel 2 (main): one thread per signature.  Per-item table {1,3,..,15}*Q in
-//     "effective affine" form on an isomorphic curve (shared Z), 33 windows of
-//     4 doublings + 2 mixed adds (Q and beta*Q share the table: x -> beta*x),
-//     then 32 mixed adds from a fixed 8-bit-window table of G (256 KB, L2
-//     resident), then the projective x comparison.  All lanes run the same
-//     double/add schedule; exceptional group-law cases go to a cold path.
+//   kernel 2 (main): one thread per signature.  Per-item table {1,3,..,31}*Q in
+//     "effective affine" form on an isomorphic curve (shared Z), 26 windows of
+//     5 doublings + 2 mixed adds (Q and beta*Q share the table: x -> beta*x),
+//     then 13 mixed adds from a fixed 20-bit-window table of G (GTAB_W), then
+//     the projective x comparison.  All lanes run the same double/add
+//     schedule; exceptional group-law cases go to a cold path.
 //
 // Off-curve public keys (the reference does not validate uncompressed keys,
 // ec/key.js:95; its output is then not a group-law function, SURVEY 8a Q1) are
@@ -45,7 +45,16 @@ enum : uint8_t {
 constexpr int PREP_WORDS = 19;
 constexpr u32 FL_INVALID = 1, FL_NEGG = 2, FL_NEG1 = 4, FL_NEG2 = 8, FL_NOG = 16;
 constexpr int PREP_BATCH = 16;          // items per thread in the batched inversion
-constexpr int QTAB_ENTRIES = 8;         // odd multiples 1,3,..,15
+// Per-item windows of the GLV halves m1, m2 (< 2^GLV_M_BITS): 16 odd multiples 1,3,..,31 of Q cost 8 more table
+// additions than 8 multiples, and save 3 doublings and 14 mixed adds over 4-bit windows.  The first QTAB_ENTRIES
+// live in the item's table in the workspace (qtab), the other QTAB_HI_ENTRIES in thread-local memory, so the
+// workspace a caller allocates keeps its size; all 16 share one Z.
+constexpr int QTAB_W = 5;
+constexpr int QTAB_ENTRIES = 8;                                // odd multiples 1,3,..,15: in the workspace
+constexpr int QTAB_HI_ENTRIES = (1 << (QTAB_W - 1)) - QTAB_ENTRIES;   // 17,19,..,31: thread-local
+constexpr int QTAB_WINDOWS = (GLV_M_BITS + QTAB_W - 1) / QTAB_W;
+static_assert(GLV_M_BITS - QTAB_W * (QTAB_WINDOWS - 1) <= QTAB_W - 1, "top digit 2m+1 must stay below 2^W");
+static_assert(QTAB_W * QTAB_WINDOWS <= 5 * 32, "m1 and m2 are stored as 5 words each");
 #if EB_K256_FQ
 constexpr int QTAB_WORDS = QTABQ_WORDS;        // per item: (x, y, beta*x) x 8, 9 limbs padded to 12 words each
 #else
@@ -58,6 +67,22 @@ constexpr int GTAB_W = EB_GW;
 constexpr int GTAB_WINDOWS = (255 + GTAB_W - 1) / GTAB_W;     // digits of m = (u1'-1)/2 (255 bits)
 constexpr int GTAB_ENTRIES = 1 << (GTAB_W - 1);               // (2i+1) * 2^(W*j) * G, i < 2^(W-1)
 static_assert(255 - GTAB_W * (GTAB_WINDOWS - 1) <= GTAB_W - 1, "top digit 2m+1 must stay below 2^W");
+
+// W-bit digit chunk at bit `pos` of the nwords-word number stored SoA from word `base` of ws
+EB_HD u32 ks_chunk(const u32* ws, size_t N, size_t i, int base, int nwords, int pos, int W) {
+  int wi = pos >> 5;
+  u32 lo = ws[(size_t)(base + wi) * N + i];
+  u32 hi = (wi + 1 < nwords) ? ws[(size_t)(base + wi + 1) * N + i] : 0u;
+  u64 both = ((u64)hi << 32) | lo;
+  return (u32)(both >> (pos & 31)) & ((1u << W) - 1);
+}
+// regular signed-odd recoding: chunk c of window w stands for the digit 2c + 1 - 2^W (top window: 2c + 1);
+// returns the table index of |digit| and whether the digit is negative
+EB_HD u32 ks_digit(u32 chunk, bool top, int W, bool* dneg) {
+  const u32 half = 1u << (W - 1);
+  *dneg = !top && chunk < half;
+  return top ? (chunk & (half - 1)) : (*dneg ? half - 1 - chunk : chunk - half);
+}
 
 struct madd_out { ge_jac r; fe h; };
 
@@ -249,9 +274,12 @@ EB_HD fe load_fe(const u32* src) { fe a; for (int i = 0; i < 8; i++) a.v[i] = sr
 // Carry-free field version: the whole double/add schedule runs on 9 x 29-bit lazy limbs (gq_k256.cuh);
 // the packed 8 x 32 form only appears at the two ends (Q in, the fixed-base table entries, R out).
 EB_HD ge_jac k256_dsm(size_t i, size_t N, const ge_aff& Q, u32 flags, const u32* ws, const u32* gtab, u32* qtab) {
-  // ---- per-item table: (2k+1)*Q, k = 0..7, as affine points on an isomorphic
+  // ---- per-item table: (2k+1)*Q, k < 16, as affine points on an isomorphic
   // curve y^2 = x^3 + 7*Zg^6 (the a = 0 formulas never use b), Zg = zglobal.
   u32* tab = qtab + (size_t)i * QTAB_WORDS;
+  alignas(16) u32 hi[QTAB_HI_ENTRIES * QTABQ_ENTRY_WORDS];
+  auto ent = [&](u32 k) { return k < QTAB_ENTRIES ? tab + QTABQ_ENTRY_WORDS * k : hi + QTABQ_ENTRY_WORDS * (k - QTAB_ENTRIES); };
+  constexpr int NE = QTAB_ENTRIES + QTAB_HI_ENTRIES;
   fqk<1> zglobal;
   {
     gq_jac Qj; Qj.x = fqk_from_fe(Q.x); Qj.y = fqk_from_fe(Q.y); Qj.z = fqk_one();
@@ -263,23 +291,23 @@ EB_HD ge_jac k256_dsm(size_t i, size_t N, const ge_aff& Q, u32 flags, const u32*
     P.y = fq_mul(Qj.y, C3);
     P.z = fqk_one();
     fq_store12(tab + 0, P.x); fq_store12(tab + FQ_PAD, P.y);
-    for (int k = 1; k < QTAB_ENTRIES; k++) {
+    for (int k = 1; k < NE; k++) {
       gq_madd_out o = gq_madd_h(P, D.x, D.y);
       P = o.r;
-      u32* e = tab + QTABQ_ENTRY_WORDS * k;
+      u32* e = ent(k);
       fq_store12(e, P.x); fq_store12(e + FQ_PAD, P.y);
       fq_store12(e + 2 * FQ_PAD, o.h);       // Z_k / Z_{k-1}, consumed below
     }
     zglobal = fq_mul(P.z, D.z);
-    // rescale every entry to Z = Z_7 and append beta*x
+    // rescale every entry to the last entry's Z and append beta*x
     const fqk<1> beta = fqk_from_fe(fe_beta());
     fqk<1> zs = fqk_one();
-    for (int k = QTAB_ENTRIES - 1; k >= 0; k--) {
-      u32* e = tab + QTABQ_ENTRY_WORDS * k;
+    for (int k = NE - 1; k >= 0; k--) {
+      u32* e = ent(k);
       fqk<1> X = fq_load12(e), Y = fq_load12(e + FQ_PAD);
       fqk<1> hk = fqk_one();
       if (k > 0) hk = fq_load12(e + 2 * FQ_PAD);
-      if (k < QTAB_ENTRIES - 1) {
+      if (k < NE - 1) {
         fqk<1> zs2 = fq_sqr(zs);
         fqk<1> zs3 = fq_mul(zs2, zs);
         X = fq_mul(X, zs2);
@@ -291,23 +319,22 @@ EB_HD ge_jac k256_dsm(size_t i, size_t N, const ge_aff& Q, u32 flags, const u32*
     }
   }
 
-  // ---- u2*Q = k1*Q + k2*(lambda*Q): 33 windows of 4 bits, regular signed-odd digits
+  // ---- u2*Q = k1*Q + k2*(lambda*Q): QTAB_WINDOWS windows of QTAB_W bits, regular signed-odd digits
   gq_jac acc;
   acc.x = fqk_one(); acc.y = fqk_one(); acc.z = fqk_zero();
-  for (int w = 32; w >= 0; w--) {
-    if (w != 32)
-      for (int d = 0; d < 4; d++) acc = gq_dbl(acc);    // (the top window starts from its first table entry)
+  for (int w = QTAB_WINDOWS - 1; w >= 0; w--) {
+    const bool top = w == QTAB_WINDOWS - 1;
+    if (!top)
+      for (int d = 0; d < QTAB_W; d++) acc = gq_dbl(acc);    // (the top window starts from its first table entry)
     for (int h = 0; h < 2; h++) {
-      u32 word = ws[(size_t)((h ? 13 : 8) + (w >> 3)) * N + i];
-      u32 nib = (word >> (4 * (w & 7))) & 15;
-      bool dneg = (w != 32) && (nib < 8);
-      u32 idx = (w == 32) ? (nib & 7) : (dneg ? 7 - nib : nib - 8);
+      bool dneg;
+      u32 idx = ks_digit(ks_chunk(ws, N, i, h ? 13 : 8, 5, QTAB_W * w, QTAB_W), top, QTAB_W, &dneg);
       bool neg = dneg != (((flags & (h ? FL_NEG2 : FL_NEG1)) != 0));
-      const u32* e = tab + QTABQ_ENTRY_WORDS * idx;
+      const u32* e = ent(idx);
       gq_aff P;
       P.x = fq_load12(e + (h ? 2 * FQ_PAD : 0));
       P.y = fq_cneg(fq_load12(e + FQ_PAD), neg);
-      if (w == 32 && h == 0) acc = gq_from_aff(P);
+      if (top && h == 0) acc = gq_from_aff(P);
       else acc = gq_madd(acc, P);
     }
   }
@@ -317,14 +344,8 @@ EB_HD ge_jac k256_dsm(size_t i, size_t N, const ge_aff& Q, u32 flags, const u32*
   // ---- u1*G from the fixed table: GTAB_WINDOWS windows of GTAB_W bits, regular signed-odd digits
   if (!(flags & FL_NOG)) {                    // Point.mul: no base-point term (uniform across a batch)
     for (int j = 0; j < GTAB_WINDOWS; j++) {
-      const int pos = GTAB_W * j;
-      u32 lo = ws[(size_t)(pos >> 5) * N + i];
-      u32 hi = ((pos >> 5) < 7) ? ws[(size_t)((pos >> 5) + 1) * N + i] : 0u;
-      u64 both = ((u64)hi << 32) | lo;
-      u32 chunk = (u32)(both >> (pos & 31)) & ((1u << GTAB_W) - 1);
-      const u32 half = 1u << (GTAB_W - 1);
-      bool dneg = (j != GTAB_WINDOWS - 1) && (chunk < half);
-      u32 idx = (j == GTAB_WINDOWS - 1) ? (chunk & (half - 1)) : (dneg ? half - 1 - chunk : chunk - half);
+      bool dneg;
+      u32 idx = ks_digit(ks_chunk(ws, N, i, 0, 8, GTAB_W * j, GTAB_W), j == GTAB_WINDOWS - 1, GTAB_W, &dneg);
       bool neg = dneg != ((flags & FL_NEGG) != 0);
       const u32* ent = gtab + ((size_t)j * GTAB_ENTRIES + idx) * 16;
       gq_aff P;
@@ -336,10 +357,14 @@ EB_HD ge_jac k256_dsm(size_t i, size_t N, const ge_aff& Q, u32 flags, const u32*
   return gq_to_jac(acc);
 }
 #else
-// Per-item table (2k+1)*Q, k = 0..7, for an ON-CURVE Q: tab[24k..24k+23] = (x, y, beta*x) as affine points on
-// the isomorphic curve y^2 = x^3 + 7*Zg^6 (the a = 0 formulas never use b); returns Zg.  Built with co-Z
-// additions (Meloni): all points of one step share a Z, so no addition needs it.
-EB_HD fe qtab_build(const ge_aff& Q, u32* tab) {
+// Per-item table (2k+1)*Q, k < QTAB_ENTRIES + NHI, for an ON-CURVE Q: entry k = (x, y, beta*x) at tab + 24k for
+// k < QTAB_ENTRIES (the item's workspace table), at hi + 24(k - QTAB_ENTRIES) after that, as affine points on the
+// isomorphic curve y^2 = x^3 + 7*Zg^6 (the a = 0 formulas never use b); returns Zg.  Built with co-Z additions
+// (Meloni): all points of one step share a Z, so no addition needs it.  NHI = 0 is the table of 4-bit windows.
+template <int NHI = 0>
+EB_HD fe qtab_build(const ge_aff& Q, u32* tab, u32* hi = nullptr) {
+  constexpr int NE = QTAB_ENTRIES + NHI;
+  auto ent = [&](int k) { return k < QTAB_ENTRIES ? tab + 24 * k : hi + 24 * (k - QTAB_ENTRIES); };
   // co-Z doubling of the affine Q (dbl-2009-l at Z = 1): D = 2Q and P = Q, both on Z = 2*y(Q), i.e. affine on
   // the curve scaled by 2*y(Q).  y(Q) != 0: the group has odd order.
   fe B = fe_sqr(Q.x);
@@ -352,7 +377,7 @@ EB_HD fe qtab_build(const ge_aff& Q, u32* tab) {
   fe Dy = fe_sub(fe_mul(M, fe_sub(S, Dx)), L8);
   fe Px = S, Py = L8;
   store_fe(tab + 0, Px); store_fe(tab + 8, Py);
-  for (int k = 1; k < QTAB_ENTRIES; k++) {
+  for (int k = 1; k < NE; k++) {
     // ZADDU: P += D with D moved to the new Z; Z_k = Z_{k-1} * h.  (2k-1)Q = +-2Q is impossible in a group of
     // large prime order, so h != 0.
     fe h = fe_sub(Px, Dx);
@@ -363,48 +388,51 @@ EB_HD fe qtab_build(const ge_aff& Q, u32* tab) {
     Px = fe_sub(fe_sub(fe_sqr(dy), W1), W2);
     Py = fe_sub(fe_mul(dy, fe_sub(W2, Px)), A2);
     Dx = W2; Dy = A2;
-    store_fe(tab + 24 * k, Px); store_fe(tab + 24 * k + 8, Py);
-    store_fe(tab + 24 * k + 16, h);                                // Z_k / Z_{k-1}, consumed below
+    u32* e = ent(k);
+    store_fe(e, Px); store_fe(e + 8, Py);
+    store_fe(e + 16, h);                                           // Z_k / Z_{k-1}, consumed below
   }
-  // rescale every entry to Z = Z_7 and append beta*x
+  // rescale every entry to the last entry's Z and append beta*x
   fe beta = fe_beta();
   fe zs = fe_one();
-  for (int k = QTAB_ENTRIES - 1; k >= 0; k--) {
-    fe X = load_fe(tab + 24 * k), Y = load_fe(tab + 24 * k + 8);
-    if (k < QTAB_ENTRIES - 1) {
+  for (int k = NE - 1; k >= 0; k--) {
+    u32* e = ent(k);
+    fe X = load_fe(e), Y = load_fe(e + 8);
+    if (k < NE - 1) {
       fe zs2 = fe_sqr(zs);
       fe zs3 = fe_mul(zs2, zs);
       X = fe_mul(X, zs2);
       Y = fe_mul(Y, zs3);
-      store_fe(tab + 24 * k, X); store_fe(tab + 24 * k + 8, Y);
+      store_fe(e, X); store_fe(e + 8, Y);
     }
-    if (k > 0) zs = fe_mul(zs, load_fe(tab + 24 * k + 16));
-    store_fe(tab + 24 * k + 16, fe_mul(X, beta));
+    if (k > 0) zs = fe_mul(zs, load_fe(e + 16));
+    store_fe(e + 16, fe_mul(X, beta));
   }
-  return fe_mul(zs, fe_dbl(Q.y));                                  // Z_7 * 2y(Q)
+  return fe_mul(zs, fe_dbl(Q.y));                                  // Z_last * 2y(Q)
 }
 
 // u1*G + u2*Q for an ON-CURVE Q, scalars as prepared by prep_thread in ws.  Jacobian result.
 EB_HD ge_jac k256_dsm(size_t i, size_t N, const ge_aff& Q, u32 flags, const u32* ws, const u32* gtab, u32* qtab) {
   u32* tab = qtab + (size_t)i * QTAB_WORDS;
-  fe zglobal = qtab_build(Q, tab);
+  alignas(16) u32 hi[QTAB_HI_ENTRIES * 24];
+  fe zglobal = qtab_build<QTAB_HI_ENTRIES>(Q, tab, hi);
 
-  // ---- u2*Q = k1*Q + k2*(lambda*Q): 33 windows of 4 bits, regular signed-odd digits
+  // ---- u2*Q = k1*Q + k2*(lambda*Q): QTAB_WINDOWS windows of QTAB_W bits, regular signed-odd digits
   ge_jac acc = jac_infinity();
-  for (int w = 32; w >= 0; w--) {
-    if (w != 32)
-      for (int d = 0; d < 4; d++) acc = jac_dbl(acc);   // (the top window starts from its first table entry)
+  for (int w = QTAB_WINDOWS - 1; w >= 0; w--) {
+    const bool top = w == QTAB_WINDOWS - 1;
+    if (!top)
+      for (int d = 0; d < QTAB_W; d++) acc = jac_dbl(acc);   // (the top window starts from its first table entry)
     for (int h = 0; h < 2; h++) {
-      u32 word = ws[(size_t)((h ? 13 : 8) + (w >> 3)) * N + i];
-      u32 nib = (word >> (4 * (w & 7))) & 15;
-      bool dneg = (w != 32) && (nib < 8);
-      u32 idx = (w == 32) ? (nib & 7) : (dneg ? 7 - nib : nib - 8);
+      bool dneg;
+      u32 idx = ks_digit(ks_chunk(ws, N, i, h ? 13 : 8, 5, QTAB_W * w, QTAB_W), top, QTAB_W, &dneg);
       bool neg = dneg != (((flags & (h ? FL_NEG2 : FL_NEG1)) != 0));
+      const u32* e = idx < QTAB_ENTRIES ? tab + 24 * idx : hi + 24 * (idx - QTAB_ENTRIES);
       ge_aff P;
-      P.x = load_fe(tab + 24 * idx + (h ? 16 : 0));
-      P.y = load_fe(tab + 24 * idx + 8);
+      P.x = load_fe(e + (h ? 16 : 0));
+      P.y = load_fe(e + 8);
       P = aff_neg_if(P, neg);
-      if (w == 32 && h == 0) acc = jac_from_aff(P);
+      if (top && h == 0) acc = jac_from_aff(P);
       else acc = jac_madd(acc, P);
     }
   }
@@ -414,14 +442,8 @@ EB_HD ge_jac k256_dsm(size_t i, size_t N, const ge_aff& Q, u32 flags, const u32*
   // ---- u1*G from the fixed table: GTAB_WINDOWS windows of GTAB_W bits, regular signed-odd digits
   if (flags & FL_NOG) return acc;             // Point.mul: no base-point term (uniform across a batch)
   for (int j = 0; j < GTAB_WINDOWS; j++) {
-    const int pos = GTAB_W * j;
-    u32 lo = ws[(size_t)(pos >> 5) * N + i];
-    u32 hi = ((pos >> 5) < 7) ? ws[(size_t)((pos >> 5) + 1) * N + i] : 0u;
-    u64 both = ((u64)hi << 32) | lo;
-    u32 chunk = (u32)(both >> (pos & 31)) & ((1u << GTAB_W) - 1);
-    const u32 half = 1u << (GTAB_W - 1);
-    bool dneg = (j != GTAB_WINDOWS - 1) && (chunk < half);
-    u32 idx = (j == GTAB_WINDOWS - 1) ? (chunk & (half - 1)) : (dneg ? half - 1 - chunk : chunk - half);
+    bool dneg;
+    u32 idx = ks_digit(ks_chunk(ws, N, i, 0, 8, GTAB_W * j, GTAB_W), j == GTAB_WINDOWS - 1, GTAB_W, &dneg);
     bool neg = dneg != ((flags & FL_NEGG) != 0);
     const u32* ent = gtab + ((size_t)j * GTAB_ENTRIES + idx) * 16;
     ge_aff P;

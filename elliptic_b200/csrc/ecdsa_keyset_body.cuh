@@ -35,22 +35,6 @@ EB_HD void ks_load_entry(u32* dst, const u32* src) {
 #endif
 }
 
-// W-bit digit chunk at bit `pos` of the nwords-word number stored SoA from word `base` of ws
-EB_HD u32 ks_chunk(const u32* ws, size_t N, size_t i, int base, int nwords, int pos, int W) {
-  int wi = pos >> 5;
-  u32 lo = ws[(size_t)(base + wi) * N + i];
-  u32 hi = (wi + 1 < nwords) ? ws[(size_t)(base + wi + 1) * N + i] : 0u;
-  u64 both = ((u64)hi << 32) | lo;
-  return (u32)(both >> (pos & 31)) & ((1u << W) - 1);
-}
-// regular signed-odd recoding: chunk c of window w stands for the digit 2c + 1 - 2^W (top window: 2c + 1);
-// returns the table index of |digit| and whether the digit is negative
-EB_HD u32 ks_digit(u32 chunk, bool top, int W, bool* dneg) {
-  const u32 half = 1u << (W - 1);
-  *dneg = !top && chunk < half;
-  return top ? (chunk & (half - 1)) : (*dneg ? half - 1 - chunk : chunk - half);
-}
-
 // keyFromPublic's verdict for key k: the decoder's throw, else pub.validate()
 EB_HD uint8_t k256_ks_classify_item(size_t k, const uint8_t* xy, const uint8_t* pre) {
   if (pre && pre[k]) return pre[k];

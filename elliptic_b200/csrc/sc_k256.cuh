@@ -123,11 +123,19 @@ EB_HD void neg256(u32* r, const u32* a) {
   sub_n<8>(r, z, a);
 }
 
-// GLV decomposition of k (< n): k = k1 + k2*lambda (mod n) with k1, k2 odd and
-// |k1|,|k2| < 2^131.  Outputs m1 = (|k1|-1)/2, m2 = (|k2|-1)/2 (5 limbs each)
-// and the signs.  Rounded quotients use the 2^384-scaled constants
-// g1 = round(2^384*b2/n), g2 = round(2^384*(-b1)/n) for the reference's own
-// basis (curves.js:189-198); the parity fix adds +-v1 / +-v2.
+// GLV decomposition of k (< n): k = k1 + k2*lambda (mod n) with k1, k2 odd.
+// Outputs m1 = (|k1|-1)/2, m2 = (|k2|-1)/2 (5 limbs each) and the signs.
+// Rounded quotients use the 2^384-scaled constants g1 = round(2^384*b2/n),
+// g2 = round(2^384*(-b1)/n) for the reference's own basis v1 = (a1, b1),
+// v2 = (a2, b2) (curves.js:189-198); the parity fix adds +-v1 / +-v2.
+//
+// Bound: before the fix (k1, k2) = -(d1 v1 + d2 v2) with |d1|, |d2| <= 1/2 (up
+// to k / 2^385 from the scaled constants).  The fix adds e1 v1, then e2 v2,
+// e1, e2 in {-1, 0, 1}, their signs set by the sign of k1 at that point.  The
+// largest |k1| and |k2| over all (d1, d2, e1, e2) are at vertices of the
+// regions those signs cut out of the square: |k1| < 2^128.12, |k2| < 2^128.66
+// (tests/test_glv_window5.py derives them), so m1, m2 < 2^GLV_M_BITS.
+constexpr int GLV_M_BITS = 128;
 EB_HD void glv_split_odd(const u32* k, u32* m1, bool* neg1, u32* m2, bool* neg2) {
   const u32 g1[8] = {0x45dbb031u, 0xe893209au, 0x71e8ca7fu, 0x3daa8a14u, 0x9284eb15u, 0xe86c90e4u, 0xa7d46bcdu, 0x3086d221u};
   const u32 g2[8] = {0x8ac47f71u, 0x1571b4aeu, 0x9df506c6u, 0x221208acu, 0x0abfe4c4u, 0x6f547fa9u, 0x010e8828u, 0xe4437ed6u};
