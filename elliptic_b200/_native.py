@@ -45,6 +45,7 @@ EXPORTS = [
     "eb200_ec_keygen_batch_dev", "eb200_ecdsa_recover_batch_dev", "eb200_ecdsa_recovery_param_batch_dev",
     "eb200_scalar_mul_batch_dev", "eb200_mul_add_batch_dev", "eb200_ecdh_derive_batch_dev", "eb200_x25519_mul_batch_dev",
     "eb200_ecdsa_verify_batch_der_dev", "eb200_eddsa_verify_batch_msgs_dev", "eb200_eddsa_sign_batch_dev",
+    "eb200_ecdsa_verify_batch_keyed_der_dev",
 ]
 
 
@@ -118,6 +119,8 @@ def load():
     lib.eb200_ecdsa_verify_keyed_workspace_bytes.restype = c.c_size_t
     lib.eb200_ecdsa_verify_keyed_workspace_bytes.argtypes = [c.c_void_p, c.c_size_t]
     lib.eb200_ecdsa_verify_batch_keyed_dev.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 7
+    lib.eb200_ecdsa_verify_batch_keyed_der_dev.argtypes = [c.c_void_p, c.c_size_t, c.c_void_p, c.c_void_p, c.c_uint64] + \
+        [c.c_void_p] * 5
     lib.eb200_keyset_dev_workspace_bytes.restype = c.c_size_t
     lib.eb200_keyset_dev_workspace_bytes.argtypes = [c.c_void_p, c.c_size_t]
     lib.eb200_scalar_mul_batch_keyed_dev.argtypes = [c.c_void_p, c.c_size_t] + [c.c_void_p] * 6

@@ -766,7 +766,7 @@ size_t fe_len(int curve) {   // field-element bytes for the selftest hooks (also
   return (curve == EB200_CURVE_P384) ? 48 : (curve == EB200_CURVE_P521) ? 72 :     // 18 limbs; p224 = 8 limbs
          ((curve >= EB200_CURVE_SECP256K1 && curve <= EB200_CURVE_CURVE25519) || curve == EB200_CURVE_P224) ? 32 : 0;
 }
-size_t curve_len(int curve) {
+constexpr size_t curve_len(int curve) {
   switch (curve) {
     case EB200_CURVE_SECP256K1: case EB200_CURVE_P256: case EB200_CURVE_ED25519: return 32;
     case EB200_CURVE_P384: return 48;
@@ -2329,9 +2329,31 @@ int keyed_verify_prep(Ctx& c, int curve, size_t m, const uint8_t* d_e, const uin
   });
 }
 
+// The launches of one keyed DER verify block whose inputs are on the device: the keyed DER decode (der + off[i] is item
+// i's encoding), or with `pre` the screened one (pre: the index-and-range screen's verdicts), then prep, keyed main
+// (between ev0 and ev1), keyed replay and verdict merge.  idx: the key indices the set may be addressed with; r, s
+// (m x len) and vd (m bytes) the decoded halves and verdicts; ws, scratch as ws_layout places them.
+int keyed_der_launches(Ctx& c, int curve, size_t m, const KeysetDev& d, const uint8_t* e, const uint8_t* der,
+                       const unsigned long long* off, const u32* idx, const uint8_t* pre, uint8_t* r, uint8_t* s, uint8_t* vd,
+                       u32* ws, u32* scratch, uint8_t* status, Launch& L, cudaEvent_t ev0, cudaEvent_t ev1) {
+  const u32 len = (u32)curve_len(curve);
+  cudaError_t err = pre ? keyset_der_decode_screened_launch(m, len, pre, der, off, idx, d, r, s, vd, L.st, &L.count)
+                        : keyset_der_decode_launch(m, len, der, off, idx, d, r, s, vd, L.st, &L.count);
+  if (err != cudaSuccess) return cuda_fail(err, pre ? "keyset_der_decode_screened_launch" : "keyset_der_decode_launch");
+  const u32* replay = nullptr;
+  int rc = keyed_verify_prep(c, curve, m, e, r, s, ws, scratch, L, &replay);
+  if (rc) return rc;
+  const KeyedVerifyArgs a{e, r, s, idx, status, ws, c.gtab[curve], replay};
+  if ((err = keyset_verify_launch(curve, m, d, a, L.st, ev0, ev1, &L.count)) != cudaSuccess)
+    return cuda_fail(err, "keyset_verify_launch");
+  if ((err = keyset_verdict_merge_launch(m, vd, status, L.st, &L.count)) != cudaSuccess)
+    return cuda_fail(err, "keyset_verdict_merge_launch");
+  return EB200_OK;
+}
+
 // Keyed verify of DER signatures, one block on one device of the set, chunked like verify_keyed_on; the variable-length
 // segments as eddsa_sign_keyed_on stages them (sig_off points at this block's first offset, offsets absolute).
-// Launches per chunk: keyed DER decode, prep, keyed main, keyed replay, verdict merge.
+// Launches per chunk: keyed_der_launches without a screen.
 int verify_keyed_der_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* sigs, const uint64_t* sig_off,
                         const u32* key_idx, uint8_t* status) {
   const int curve = ks->curve;
@@ -2365,18 +2387,9 @@ int verify_keyed_der_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t*
     [&](size_t lo, size_t m, Launch& L, int slot, int k) {
       u32* ws = (u32*)(c.d_ws + (size_t)slot * ws_slot + W.ws);
       u32* scratch = (u32*)(c.d_ws + (size_t)slot * ws_slot + W.scratch);
-      cudaError_t err = keyset_der_decode_launch(m, (u32)len, d_sig - sig_off[0], d_off + lo, d_idx + lo, d, d_r + lo * len,
-                                                 d_s + lo * len, d_vd + lo, L.st, &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "keyset_der_decode_launch");
-      const u32* replay = nullptr;
-      int rc2 = keyed_verify_prep(c, curve, m, d_e + lo * len, d_r + lo * len, d_s + lo * len, ws, scratch, L, &replay);
-      if (rc2) return rc2;
-      const KeyedVerifyArgs a{d_e + lo * len, d_r + lo * len, d_s + lo * len, d_idx + lo, c.d_status + lo, ws, c.gtab[curve], replay};
-      if ((err = keyset_verify_launch(curve, m, d, a, L.st, c.ev_k0[k], c.ev_k1[k], &L.count)) != cudaSuccess)
-        return cuda_fail(err, "keyset_verify_launch");
-      if ((err = keyset_verdict_merge_launch(m, d_vd + lo, c.d_status + lo, L.st, &L.count)) != cudaSuccess)
-        return cuda_fail(err, "keyset_verdict_merge_launch");
-      return EB200_OK;
+      return keyed_der_launches(c, curve, m, d, d_e + lo * len, d_sig - sig_off[0], d_off + lo, d_idx + lo, nullptr,
+                                d_r + lo * len, d_s + lo * len, d_vd + lo, ws, scratch, c.d_status + lo, L, c.ev_k0[k],
+                                c.ev_k1[k]);
     },
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {status + lo, c.d_status + lo, m};
@@ -2402,6 +2415,15 @@ KeyedDevWs keyed_dev_ws(size_t n, size_t body) {
 size_t keyed_mul_ws_bytes(int curve, size_t n) {
   return align256(ws_layout(curve, n).qtab + 3 * (size_t)keyset_geom(curve).limbs * n * 4);
 }
+
+// eb200_ecdsa_verify_batch_keyed_der_dev keeps the decoded r, s (len bytes each) and the index-and-range screen's verdict
+// of every item in the Jacobian-result region of keyed_mul_ws_bytes (3 x limbs words per item), which starts behind the
+// prep words and inversion scratch that the unchanged prep writes; so the keyed workspace size serves it unchanged.
+constexpr bool keyed_der_fits_jacobian(int curve) { return 2 * curve_len(curve) + 1 <= 3 * (size_t)keyset_geom(curve).limbs * 4; }
+static_assert(keyed_der_fits_jacobian(EB200_CURVE_SECP256K1) && keyed_der_fits_jacobian(EB200_CURVE_P256) &&
+              keyed_der_fits_jacobian(EB200_CURVE_P384) && keyed_der_fits_jacobian(EB200_CURVE_P521) &&
+              keyed_der_fits_jacobian(EB200_CURVE_P192) && keyed_der_fits_jacobian(EB200_CURVE_P224),
+              "r, s and the screen verdicts of the keyed DER device form must fit the keyed workspace's Jacobian region");
 
 // The launches of one keyed mul / mulAdd / derive block whose inputs are on the device (k1 == NULL: no base-point term):
 // prep_scalars, keyed main (between ev0 and ev1), normalisation, then the keyed replay (derive: the status map).
@@ -2935,6 +2957,25 @@ int eb200_ecdsa_verify_batch_keyed_dev(const eb200_keyset* ks, size_t n, const u
       if ((err = keyset_verdict_merge_launch(n, vd, d_status, L.st, &L.count)) != cudaSuccess)
         return cuda_fail(err, "keyset_verdict_merge_launch");
       return EB200_OK;
+    });
+}
+
+// workspace body (keyed_mul_ws_bytes): [prep words | inversion scratch | r (n x len) | s (n x len) | screen verdicts (n)],
+// the last three inside the Jacobian-result region (keyed_der_fits_jacobian)
+int eb200_ecdsa_verify_batch_keyed_der_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_e, const uint8_t* d_sigs,
+                                           uint64_t sigs_len, const uint64_t* d_sig_off, const uint32_t* d_key_idx,
+                                           uint8_t* d_status, void* d_workspace, void* stream) {
+  return keyed_dev_run(ks, KK_ECDSA, n, d_e && d_sig_off && d_key_idx && (d_sigs || !sigs_len), d_status, d_workspace, stream,
+    [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
+      const int curve = ks->curve;
+      const size_t len = curve_len(curve);
+      const WsLayout W = ws_layout(curve, n);
+      uint8_t *r = body + W.qtab, *s = r + len * n, *pre = s + len * n;
+      cudaError_t err = keyset_index_range_screen_launch(n, d_key_idx, ks->m, d_sig_off, sigs_len, idx, pre, L.st, &L.count);
+      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_range_screen_launch");
+      return keyed_der_launches(c, curve, n, d, d_e, d_sigs, (const unsigned long long*)d_sig_off, idx, pre,
+                                r, s, vd, (u32*)(body + W.ws), (u32*)(body + W.scratch), d_status, L, c.ev[EV_MAIN_BEGIN],
+                                c.ev[EV_MAIN_END]);
     });
 }
 

@@ -50,6 +50,11 @@ cudaError_t keyset_verify_launch(int curve, size_t n, const KeysetDev& k, const 
 cudaError_t keyset_der_decode_launch(size_t n, uint32_t len, const uint8_t* der, const unsigned long long* off,
                                      const uint32_t* key_idx, const KeysetDev& k, uint8_t* r, uint8_t* s, uint8_t* verdict,
                                      cudaStream_t st, unsigned* launches);
+// The DER decode behind the index-and-range screen: pre holds that screen's verdicts and idx its screened indices; an
+// item with a non-zero pre reads nothing, gets r = s = 0 and verdict pre[i], any other is decoded as above.
+cudaError_t keyset_der_decode_screened_launch(size_t n, uint32_t len, const uint8_t* pre, const uint8_t* der,
+                                              const unsigned long long* off, const uint32_t* idx, const KeysetDev& k,
+                                              uint8_t* r, uint8_t* s, uint8_t* verdict, cudaStream_t st, unsigned* launches);
 // Index screen: idx_out[i] = key_idx[i] when it is below m, else 0 with verdict EB200_ST_BAD_KEY_INDEX.
 cudaError_t keyset_index_screen_launch(size_t n, const uint32_t* key_idx, size_t m, uint32_t* idx_out, uint8_t* verdict,
                                        cudaStream_t st, unsigned* launches);

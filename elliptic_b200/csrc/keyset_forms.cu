@@ -1,6 +1,7 @@
 // keyset_forms.cu -- the kernels that frame the unchanged keyed ECDSA verify (keyset.cu) for
-// eb200_ecdsa_verify_batch_keyed_der (DER decode with the key's verdict, in front of the unchanged prep) and
-// eb200_ecdsa_verify_batch_keyed_dev (index screen in front of it), and the verdict merge that both run behind the keyed
+// eb200_ecdsa_verify_batch_keyed_der (DER decode with the key's verdict, in front of the unchanged prep),
+// eb200_ecdsa_verify_batch_keyed_dev (index screen in front of it) and eb200_ecdsa_verify_batch_keyed_der_dev (the same
+// DER decode behind the index-and-range screen), and the verdict merge that all three run behind the keyed
 // replay; and those that frame the unchanged keyed kernels of the other device-pointer keyed calls: the index, scalar
 // and message-range screens, the merge that also zeroes outputs, and the screened hash and challenge kernels (the
 // screened nonce kernel is in keyset_forms_nonce.cu).  Bodies: keyset_forms_body.cuh.
@@ -27,6 +28,14 @@ keyset_der_decode_kernel(size_t N, u32 len, const uint8_t* __restrict__ der, con
                          uint8_t* __restrict__ s, uint8_t* __restrict__ verdict) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < N) verdict[i] = ks_der_verdict_item(i, len, der, off, key_idx, kst, r, s);
+}
+__global__ void __launch_bounds__(128)
+keyset_der_decode_screened_kernel(size_t N, u32 len, const uint8_t* __restrict__ pre, const uint8_t* __restrict__ der,
+                                  const unsigned long long* __restrict__ off, const u32* __restrict__ idx,
+                                  const uint8_t* __restrict__ kst, uint8_t* __restrict__ r, uint8_t* __restrict__ s,
+                                  uint8_t* __restrict__ verdict) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < N) verdict[i] = ks_der_screened_item(i, len, pre, der, off, idx, kst, r, s);
 }
 __global__ void __launch_bounds__(128)
 keyset_index_screen_kernel(size_t N, const u32* __restrict__ key_idx, size_t m, u32* __restrict__ idx_out,
@@ -89,6 +98,13 @@ cudaError_t keyset_der_decode_launch(size_t n, uint32_t len, const uint8_t* der,
                                      const uint32_t* key_idx, const KeysetDev& k, uint8_t* r, uint8_t* s, uint8_t* verdict,
                                      cudaStream_t st, unsigned* launches) {
   keyset_der_decode_kernel<<<blocks128(n), 128, 0, st>>>(n, len, der, off, key_idx, k.kst, r, s, verdict);
+  return counted(launches);
+}
+
+cudaError_t keyset_der_decode_screened_launch(size_t n, uint32_t len, const uint8_t* pre, const uint8_t* der,
+                                              const unsigned long long* off, const uint32_t* idx, const KeysetDev& k,
+                                              uint8_t* r, uint8_t* s, uint8_t* verdict, cudaStream_t st, unsigned* launches) {
+  keyset_der_decode_screened_kernel<<<blocks128(n), 128, 0, st>>>(n, len, pre, der, off, idx, k.kst, r, s, verdict);
   return counted(launches);
 }
 

@@ -38,6 +38,18 @@ EB_HD uint8_t ks_index_screen_item(size_t i, const u32* key_idx, size_t m, u32* 
   return bad ? (uint8_t)EB200_ST_BAD_KEY_INDEX : 0;
 }
 
+// ks_der_verdict_item behind the index-and-range screen (ks_index_range_screen_item), for the keyed DER verify on
+// device pointers: pre[i] is the screen's verdict and idx the screened indices.  A screened item reads no byte of its
+// range, gets r = s = 0 and keeps its verdict; any other is decoded with its key's verdict exactly as there.  So the
+// precedence is BAD_KEY_INDEX, BAD_ITEM, the key's import throw, THROW_SIG_FORMAT.
+EB_HD uint8_t ks_der_screened_item(size_t i, u32 len, const uint8_t* pre, const uint8_t* der, const unsigned long long* off,
+                                   const u32* idx, const uint8_t* kst, uint8_t* r, uint8_t* s) {
+  const uint8_t v = pre[i];
+  if (!v) return ks_der_verdict_item(i, len, der, off, idx, kst, r, s);
+  for (u32 k = 0; k < len; k++) r[(size_t)len * i + k] = s[(size_t)len * i + k] = 0;
+  return v;
+}
+
 // Item i after the keyed replay: a non-zero verdict replaces the keyed status.
 EB_HD void ks_verdict_merge_item(size_t i, const uint8_t* verdict, uint8_t* status) {
   const uint8_t v = verdict[i];

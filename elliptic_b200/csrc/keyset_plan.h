@@ -11,7 +11,7 @@
 // secp256k1 (beta * x is recomputed per lookup, not stored), bits(n) - 1 otherwise.  windows = floor(mbits / W) + 1
 // keeps the top digit 2 m_top + 1 below 2^W, i.e. positive, for every W.
 struct KeysetGeom { int mbits, limbs; };
-static inline KeysetGeom keyset_geom(int curve) {
+static constexpr KeysetGeom keyset_geom(int curve) {
   switch (curve) {
     case EB200_CURVE_SECP256K1: return {131, 8};
     case EB200_CURVE_P256: return {255, 8};

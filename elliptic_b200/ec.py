@@ -263,7 +263,130 @@ class _KeyObjects:
         return KeySet(self, keys, enc, table_bits)
 
 
-class EC(_KeyObjects):
+class _TensorForms:
+    """The device-buffer calls on CUDA tensors, on the caller's stream (conventions: _tensors); EC inherits them."""
+
+    def _tensor_call(self, name, fn, specs, head, outs, zeroed=False, ws=True):
+        """Checks specs, then fn(*head(n), *outs, status[, workspace], stream) with outs new (n, ...) uint8 tensors (zeroed:
+        filled with zeros first).  Returns the outputs and the status."""
+        from . import _tensors as T
+        if self.name == "curve25519" and name not in ("derive_batch_tensors", "x_mul_batch_tensors"):
+            raise EllipticError("%s: not available on curve25519" % name)
+        n, dev = T.check(name, specs)
+        res = [(T.zeros if zeroed else T.empty)(dev, n, *shape) for shape in outs] + [T.empty(dev, n)]
+        T.launch(fn, dev, head(n) + res, T.ws_unkeyed(self._c["id"], n) if ws else None)
+        return res
+
+    def _rows(self, *named, width=None):
+        from . import _tensors as T
+        return [(a, t, T.ROWS, width or self._len) for a, t in named]
+
+    def verify_batch_tensors(self, e, r, s, pub, pub_fmt=nat.PUB_XY):
+        """verify_batch_packed on CUDA tensors (eb200_ecdsa_verify_batch_dev): e, r, s (n, len), pub (n, k) in pub_fmt.
+        Returns the (n,) statuses."""
+        if pub_fmt not in (nat.PUB_XY, nat.PUB_SEC1_65, nat.PUB_SEC1_33):
+            raise ValueError("verify_batch_tensors: unknown pub_fmt %r" % (pub_fmt,))
+        specs = self._rows(("e", e), ("r", r), ("s", s)) + self._rows(("pub", pub), width=self._pub_bytes(pub_fmt))
+        (st,) = self._tensor_call("verify_batch_tensors", "eb200_ecdsa_verify_batch_dev", specs,
+                                  lambda n: [self._c["id"], n, e, r, s, pub, pub_fmt], [])
+        return st
+
+    def verify_batch_der_tensors(self, e, sigs, sig_off, pub, pub_fmt=nat.PUB_XY):
+        """verify_batch_der_packed on CUDA tensors (eb200_ecdsa_verify_batch_der_dev): e (n, len), the DER encodings back
+        to back in sigs (1-D uint8) with (n + 1,) int64 offsets, pub (n, k) in pub_fmt.  Returns the (n,) statuses; an
+        item whose range decreases or ends past sigs gets ST_BAD_ITEM."""
+        from . import _tensors as T
+        if pub_fmt not in (nat.PUB_XY, nat.PUB_SEC1_65, nat.PUB_SEC1_33):
+            raise ValueError("verify_batch_der_tensors: unknown pub_fmt %r" % (pub_fmt,))
+        specs = self._rows(("e", e)) + [("sigs", sigs, T.BYTES, 0), ("sig_off", sig_off, T.OFF, 0)] + \
+            self._rows(("pub", pub), width=self._pub_bytes(pub_fmt))
+        (st,) = self._tensor_call("verify_batch_der_tensors", "eb200_ecdsa_verify_batch_der_dev", specs,
+                                  lambda n: [self._c["id"], n, e, sigs, sigs.numel(), sig_off, pub, pub_fmt], [])
+        return st
+
+    def sign_batch_tensors(self, e, priv, canonical=False, k=None, pers=None):
+        """One batch of EC.sign on CUDA tensors: e (n, len) truncated hashes (< n), priv (n, len) reduced mod n, as
+        eb200_ecdsa_sign_batch takes them.  k: (n, len) nonces for one attempt (eb200_ecdsa_sign_batch_k_dev; a RETRY
+        item's r, s and recid stay zero), or pers: the personalisation bytes as a 1-D uint8 tensor
+        (eb200_ecdsa_sign_batch_pers_dev); neither: RFC 6979 nonces.  Returns (r, s, recid, status)."""
+        from . import _tensors as T
+        if self.name not in _XY:
+            raise EllipticError("sign_batch_tensors: not available on " + self.name)
+        if k is not None and pers is not None:
+            raise ValueError("sign_batch_tensors: k and pers exclude each other")
+        cid, flags = self._c["id"], 1 if canonical else 0
+        specs = self._rows(("e", e), ("priv", priv), ("k", k)) + [("pers", pers, T.BYTES, 0)]
+        outs = [(self._len,), (self._len,), ()]
+        if k is not None:
+            return self._tensor_call("sign_batch_tensors", "eb200_ecdsa_sign_batch_k_dev", specs,
+                                     lambda n: [cid, n, e, priv, k, flags], outs, zeroed=True)
+        if pers is not None:
+            return self._tensor_call("sign_batch_tensors", "eb200_ecdsa_sign_batch_pers_dev", specs,
+                                     lambda n: [cid, n, e, priv, pers, pers.numel(), flags], outs)
+        return self._tensor_call("sign_batch_tensors", "eb200_ecdsa_sign_batch_dev", specs,
+                                 lambda n: [cid, n, e, priv, flags], outs)
+
+    def gen_key_pair_batch_tensors(self, entropy, pers=None):
+        """gen_key_pair_batch on CUDA tensors (eb200_ec_keygen_batch_dev): entropy (n, k) uint8, k >= 24, one row per key;
+        pers: the personalisation bytes as a 1-D uint8 tensor, or None.  Returns (priv (n, len), pub (n, 2 len), status)."""
+        from . import _tensors as T
+        if self.name not in _XY:
+            raise EllipticError("gen_key_pair_batch_tensors: not available on " + self.name)
+        specs = [("entropy", entropy, T.ROWS, None), ("pers", pers, T.BYTES, 0)]
+        return self._tensor_call("gen_key_pair_batch_tensors", "eb200_ec_keygen_batch_dev", specs,
+                                 lambda n: [self._c["id"], n, entropy, entropy.shape[1], pers,
+                                            0 if pers is None else pers.numel()], [(self._len,), (2 * self._len,)])
+
+    def recover_pub_key_batch_tensors(self, e, r, s, recid):
+        """recoverPubKey on CUDA tensors (eb200_ecdsa_recover_batch_dev): e, r, s (n, len) as recover_pub_key_batch's call
+        takes them, recid (n,) uint8.  Returns (points (n, 2 len), status)."""
+        from . import _tensors as T
+        specs = self._rows(("e", e), ("r", r), ("s", s)) + [("recid", recid, T.VEC, 0)]
+        return self._tensor_call("recover_pub_key_batch_tensors", "eb200_ecdsa_recover_batch_dev", specs,
+                                 lambda n: [self._c["id"], n, e, r, s, recid], [(2 * self._len,)])
+
+    def get_key_recovery_param_batch_tensors(self, e, r, s, q):
+        """getKeyRecoveryParam on CUDA tensors (eb200_ecdsa_recovery_param_batch_dev): e, r, s (n, len) as
+        get_key_recovery_param_batch's call takes them, q (n, 2 len) the points.  Returns (recid (n,), status)."""
+        specs = self._rows(("e", e), ("r", r), ("s", s)) + self._rows(("q", q), width=2 * self._len)
+        return self._tensor_call("get_key_recovery_param_batch_tensors", "eb200_ecdsa_recovery_param_batch_dev",
+                                 specs, lambda n: [self._c["id"], n, e, r, s, q], [()])
+
+    def mul_batch_tensors(self, k, points=None):
+        """Point.mul on CUDA tensors (eb200_scalar_mul_batch_dev): k (n, len) scalars, points (n, 2 len) x || y, or None
+        for the base point.  Returns (out (n, 2 len), status)."""
+        specs = self._rows(("k", k)) + self._rows(("points", points), width=2 * self._len)
+        return self._tensor_call("mul_batch_tensors", "eb200_scalar_mul_batch_dev", specs,
+                                 lambda n: [self._c["id"], n, k, points], [(2 * self._len,)])
+
+    def mul_add_batch_tensors(self, k1, k2, points):
+        """G.mulAdd(k1, P, k2) on CUDA tensors (eb200_mul_add_batch_dev): k1, k2 (n, len), points (n, 2 len).  Returns
+        (out (n, 2 len), status)."""
+        specs = self._rows(("k1", k1), ("k2", k2)) + self._rows(("points", points), width=2 * self._len)
+        return self._tensor_call("mul_add_batch_tensors", "eb200_mul_add_batch_dev", specs,
+                                 lambda n: [self._c["id"], n, k1, k2, points], [(2 * self._len,)])
+
+    def derive_batch_tensors(self, priv, pub):
+        """ECDH on CUDA tensors: priv (n, len) reduced mod n; pub (n, 2 len) peer points (eb200_ecdh_derive_batch_dev), or
+        on curve25519 (n, 32) peer x (eb200_x25519_derive_batch_dev), as derive_batch_packed.  Returns (x (n, len),
+        status)."""
+        if self.name == "curve25519":
+            return self._tensor_call("derive_batch_tensors", "eb200_x25519_derive_batch_dev",
+                                     self._rows(("priv", priv), ("pub", pub)), lambda n: [n, priv, pub], [(32,)], ws=False)
+        specs = self._rows(("priv", priv)) + self._rows(("pub", pub), width=2 * self._len)
+        return self._tensor_call("derive_batch_tensors", "eb200_ecdh_derive_batch_dev", specs,
+                                 lambda n: [self._c["id"], n, priv, pub], [(self._len,)])
+
+    def x_mul_batch_tensors(self, k, px):
+        """curve25519 x_mul_batch on CUDA tensors (eb200_x25519_mul_batch_dev): k, px (n, 32) big-endian.  Returns (x (n,
+        32), status)."""
+        if self.name != "curve25519":
+            raise EllipticError("x_mul_batch_tensors: curve25519 only")
+        return self._tensor_call("x_mul_batch_tensors", "eb200_x25519_mul_batch_dev",
+                                 self._rows(("k", k), ("px", px)), lambda n: [n, k, px], [(32,)], ws=False)
+
+
+class EC(_KeyObjects, _TensorForms):
     def __init__(self, curve="secp256k1", device=0):
         if curve not in _CURVES:
             raise EllipticError("Unknown curve " + str(curve))   # ec/index.js:19-20
@@ -917,6 +1040,64 @@ class KeySet(_NativeSets):
                 st[i] = v
         return st
 
+    # ---- tensor forms: the keyed device-buffer calls on CUDA tensors (conventions: _tensors) -------------------------
+    def _where_on(self, dev):
+        """_where on `dev` as (native set of each key, its index there, the native sets' sizes), built once per device."""
+        cache = self.__dict__.setdefault("_where_dev", {})
+        if dev not in cache:
+            import torch
+            w = torch.from_numpy(self._where.astype(np.int64)).to(dev)
+            cache[dev] = (w[:, 0].contiguous(), w[:, 1].contiguous(),
+                          np.bincount(self._where[:, 0], minlength=len(self._sets)).tolist())
+        return cache[dev]
+
+    def _keyed_tensors(self, name, fn, specs, ins, key_idx, outs):
+        from . import _tensors as T
+        n, dev = T.check(name, specs + [("key_idx", key_idx, T.IDX, 0)], self._sets)
+        return T.keyed(name, self._sets, len(self.status), self._where_on if len(self._sets) > 1 else None, fn, n, dev,
+                       ins, key_idx, [(n,) + o for o in outs])
+
+    def _rows(self, *named, width=None):
+        from . import _tensors as T
+        return [(a, t, T.ROWS, width or self._ec._len) for a, t in named]
+
+    def verify_batch_tensors(self, e, r, s, key_idx):
+        """verify_batch_packed on CUDA tensors (eb200_ecdsa_verify_batch_keyed_dev).  Returns the (n,) statuses."""
+        (st,) = self._keyed_tensors("verify_batch_tensors", "eb200_ecdsa_verify_batch_keyed_dev",
+                                    self._rows(("e", e), ("r", r), ("s", s)), [e, r, s], key_idx, [])
+        return st
+
+    def verify_batch_der_tensors(self, e, sigs, sig_off, key_idx):
+        """verify_batch_der_packed on CUDA tensors (eb200_ecdsa_verify_batch_keyed_der_dev): e (n, len), the DER encodings
+        back to back in sigs (1-D uint8) with (n + 1,) int64 offsets.  Returns the (n,) statuses; a range that decreases
+        or ends past sigs gets ST_BAD_ITEM."""
+        from . import _tensors as T
+        specs = self._rows(("e", e)) + [("sigs", sigs, T.BYTES, 0), ("sig_off", sig_off, T.OFF, 0)]
+        (st,) = self._keyed_tensors("verify_batch_der_tensors", "eb200_ecdsa_verify_batch_keyed_der_dev", specs,
+                                    [e, sigs, sigs.numel(), sig_off], key_idx, [])
+        return st
+
+    def mul_batch_tensors(self, k, key_idx):
+        """mul_batch_packed on CUDA tensors (eb200_scalar_mul_batch_keyed_dev).  Returns (out (n, 2 len), status)."""
+        return self._keyed_tensors("mul_batch_tensors", "eb200_scalar_mul_batch_keyed_dev", self._rows(("k", k)),
+                                   [k], key_idx, [(2 * self._ec._len,)])
+
+    def mul_add_batch_tensors(self, k1, k2, key_idx):
+        """mul_add_batch_packed on CUDA tensors (eb200_mul_add_batch_keyed_dev).  Returns (out (n, 2 len), status)."""
+        return self._keyed_tensors("mul_add_batch_tensors", "eb200_mul_add_batch_keyed_dev",
+                                   self._rows(("k1", k1), ("k2", k2)), [k1, k2], key_idx, [(2 * self._ec._len,)])
+
+    def derive_batch_tensors(self, priv, key_idx):
+        """derive_batch_packed on CUDA tensors (eb200_ecdh_derive_batch_keyed_dev).  Returns (x (n, len), status)."""
+        return self._keyed_tensors("derive_batch_tensors", "eb200_ecdh_derive_batch_keyed_dev",
+                                   self._rows(("priv", priv)), [priv], key_idx, [(self._ec._len,)])
+
+    def recovery_param_batch_tensors(self, e, r, s, key_idx):
+        """recovery_param_batch_packed on CUDA tensors (eb200_ecdsa_recovery_param_batch_keyed_dev).  Returns (recid (n,),
+        status)."""
+        return self._keyed_tensors("recovery_param_batch_tensors", "eb200_ecdsa_recovery_param_batch_keyed_dev",
+                                   self._rows(("e", e), ("r", r), ("s", s)), [e, r, s], key_idx, [()])
+
 
 class X25519KeySet(_NativeSets):
     """curve25519 peer keys imported once (eb200_x25519_keyset_create) and kept on the GPU as their edwards25519 images
@@ -970,3 +1151,11 @@ class X25519KeySet(_NativeSets):
             raise ValueError("derive_batch: one key index per private key")
         out, st = self.derive_batch_packed(_pack((_bn(k) % self._ec.n for k in privs), 32), key_idx)
         return _unpack(out, 32, st), st
+
+    def derive_batch_tensors(self, priv, key_idx):
+        """derive_batch_packed on CUDA tensors (eb200_x25519_derive_batch_keyed_dev): priv (n, 32) big-endian; a priv >= n
+        gets ST_BAD_ITEM.  Returns (x (n, 32), status)."""
+        from . import _tensors as T
+        n, dev = T.check("derive_batch_tensors", [("priv", priv, T.ROWS, 32), ("key_idx", key_idx, T.IDX, 0)], self._sets)
+        return T.keyed("derive_batch_tensors", self._sets, len(self.status), None,
+                       "eb200_x25519_derive_batch_keyed_dev", n, dev, [priv], key_idx, [(n, 32)])

@@ -34,7 +34,44 @@ class _EdKeyObjects:
         return EdSigningSet(self, secrets)
 
 
-class EDDSA(_EdKeyObjects):
+class _EdTensorForms:
+    """The EdDSA device-buffer calls on CUDA tensors, on the caller's stream (conventions: _tensors); EDDSA inherits
+    them."""
+
+    def verify_batch_tensors(self, R, S, A, h):
+        """verify_batch_packed on CUDA tensors (eb200_eddsa_verify_batch_dev): R, S, A, h (n, 32).  Returns the statuses."""
+        from . import _tensors as T
+        n, dev = T.check("verify_batch_tensors", [(a, t, T.ROWS, 32) for a, t in (("R", R), ("S", S), ("A", A), ("h", h))])
+        st = T.empty(dev, n)
+        T.launch("eb200_eddsa_verify_batch_dev", dev, [n, R, S, A, h, st], T.ws_unkeyed(nat.CURVE_ED25519, n))
+        return st
+
+    def verify_batch_msgs_tensors(self, R, S, A, msgs, msg_off):
+        """verify_batch_msgs_packed on CUDA tensors (eb200_eddsa_verify_batch_msgs_dev): R, S, A (n, 32), the messages
+        back to back in msgs (1-D uint8) with (n + 1,) int64 offsets.  Returns the statuses (ST_BAD_ITEM for a range that
+        decreases or ends past msgs)."""
+        from . import _tensors as T
+        n, dev = T.check("verify_batch_msgs_tensors", [(a, t, T.ROWS, 32) for a, t in (("R", R), ("S", S), ("A", A))] +
+                         [("msgs", msgs, T.BYTES, 0), ("msg_off", msg_off, T.OFF, 0)])
+        st = T.empty(dev, n)
+        T.launch("eb200_eddsa_verify_batch_msgs_dev", dev, [n, R, S, A, msgs, msgs.numel(), msg_off, st],
+                 T.ws_unkeyed(nat.CURVE_ED25519, n))
+        return st
+
+    def sign_batch_tensors(self, secrets, msgs, msg_off, want_pub=False):
+        """sign_batch_packed on CUDA tensors (eb200_eddsa_sign_batch_dev): secrets (n, 32), the messages back to back in
+        msgs (1-D uint8) with (n + 1,) int64 offsets.  Returns (sig (n, 64), status), or (sig, pub (n, 32), status) with
+        want_pub; a range that decreases or ends past msgs gets ST_BAD_ITEM and zeroed rows."""
+        from . import _tensors as T
+        n, dev = T.check("sign_batch_tensors", [("secrets", secrets, T.ROWS, 32), ("msgs", msgs, T.BYTES, 0),
+                                                ("msg_off", msg_off, T.OFF, 0)])
+        sig, pub, st = T.empty(dev, n, 64), T.empty(dev, n, 32) if want_pub else None, T.empty(dev, n)
+        T.launch("eb200_eddsa_sign_batch_dev", dev, [n, secrets, msgs, msgs.numel(), msg_off, sig, pub, st],
+                 T.ws_unkeyed(nat.CURVE_ED25519, n))
+        return (sig, pub, st) if want_pub else (sig, st)
+
+
+class EDDSA(_EdKeyObjects, _EdTensorForms):
     def __init__(self, curve="ed25519", device=0):
         if curve != "ed25519":
             raise EllipticError("only tested with ed25519 so far")      # eddsa/index.js:12
@@ -238,6 +275,29 @@ class EdKeySet(_NativeSets):
         h = _pack([ed.hash_int(sig[i][:32], self._A[idx[i]], ms[i]) for i in range(n)], 32, "little")
         return self.verify_batch_packed(R, S, h, idx)
 
+    # ---- tensor forms: the keyed device-buffer calls on CUDA tensors (conventions: _tensors) -------------------------
+    def _keyed_tensors(self, name, fn, specs, ins, key_idx, outs):
+        from . import _tensors as T
+        n, dev = T.check(name, specs + [("key_idx", key_idx, T.IDX, 0)], self._sets)
+        return T.keyed(name, self._sets, len(self.status), None, fn, n, dev, ins, key_idx, [(n,) + o for o in outs])
+
+    def verify_batch_tensors(self, R, S, h, key_idx):
+        """verify_batch_packed on CUDA tensors (eb200_eddsa_verify_batch_keyed_dev): R, S, h (n, 32); an h >= n gets
+        ST_BAD_ITEM.  Returns the statuses."""
+        from . import _tensors as T
+        (st,) = self._keyed_tensors("verify_batch_tensors", "eb200_eddsa_verify_batch_keyed_dev",
+                                    [(a, t, T.ROWS, 32) for a, t in (("R", R), ("S", S), ("h", h))], [R, S, h], key_idx, [])
+        return st
+
+    def verify_batch_msgs_tensors(self, R, S, msgs, msg_off, key_idx):
+        """verify_batch_msgs_packed on CUDA tensors (eb200_eddsa_verify_batch_keyed_msgs_dev): R, S (n, 32), the messages
+        back to back in msgs (1-D uint8) with (n + 1,) int64 offsets.  Returns the statuses."""
+        from . import _tensors as T
+        specs = [("R", R, T.ROWS, 32), ("S", S, T.ROWS, 32), ("msgs", msgs, T.BYTES, 0), ("msg_off", msg_off, T.OFF, 0)]
+        (st,) = self._keyed_tensors("verify_batch_msgs_tensors", "eb200_eddsa_verify_batch_keyed_msgs_dev", specs,
+                                    [R, S, msgs, msgs.numel(), msg_off], key_idx, [])
+        return st
+
 
 class EdSigningSet(_NativeSets):
     """ed25519 signing keys imported once from their 32-byte secrets (eb200_eddsa_signing_set_create): the GPU keeps each
@@ -301,3 +361,12 @@ class EdSigningSet(_NativeSets):
             raise ValueError("messages and key_idx must have the same length")
         sig = self.sign_batch_packed(*_blob([_parse_bytes(m) for m in messages]), key_idx)
         return [sig[i].tobytes() for i in range(n)]
+
+    def sign_batch_tensors(self, msgs, msg_off, key_idx):
+        """sign_batch_packed on CUDA tensors (eb200_eddsa_sign_batch_keyed_dev): the messages back to back in msgs (1-D
+        uint8) with (n + 1,) int64 offsets, key_idx (n,).  Returns (sig (n, 64), status)."""
+        from . import _tensors as T
+        n, dev = T.check("sign_batch_tensors", [("key_idx", key_idx, T.IDX, 0), ("msgs", msgs, T.BYTES, 0),
+                                                ("msg_off", msg_off, T.OFF, 0)], self._sets)
+        return T.keyed("sign_batch_tensors", self._sets, len(self.public), None, "eb200_eddsa_sign_batch_keyed_dev",
+                       n, dev, [msgs, msgs.numel(), msg_off], key_idx, [(n, 64)])

@@ -488,6 +488,16 @@ int eb200_x25519_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint
  * main kernel (the nonce kernel for sign); launches as stated per call. */
 size_t eb200_keyset_dev_workspace_bytes(const eb200_keyset* ks, size_t n);   /* 0 for NULL; for an ECDSA set at least
                                                                                 eb200_ecdsa_verify_keyed_workspace_bytes */
+/* Keyed verify of DER signatures (eb200_ecdsa_verify_batch_keyed_der) on device pointers: d_e (n x len), d_key_idx, and
+ * the sigs_len bytes at d_sigs (NULL only when sigs_len = 0) with n + 1 offsets d_sig_off into them.  For every item the
+ * host form accepts, d_status[i] is byte for byte what the host form writes, in its precedence: the key's import throw,
+ * THROW_SIG_FORMAT, FALSE for r or s out of range, then the keyed verdict (for an off-curve key, the keyed replay's).
+ * Otherwise BAD_KEY_INDEX for d_key_idx[i] >= m, else BAD_ITEM for a range that decreases or ends past sigs_len, which is
+ * never read; BAD_ITEM takes precedence over a key's throw, as in eb200_ecdsa_verify_batch_der_dev.  main = the keyed
+ * main kernel; launches = 6: index and range screen, screened keyed DER decode, prep, keyed main, keyed replay, merge. */
+int eb200_ecdsa_verify_batch_keyed_der_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_e, const uint8_t* d_sigs,
+                                           uint64_t sigs_len, const uint64_t* d_sig_off, const uint32_t* d_key_idx,
+                                           uint8_t* d_status, void* d_workspace, void* stream);
 /* ECDSA sets.  launches = 6: index screen, scalar prep, keyed main, normalisation, keyed replay (derive: the status
  * map), merge. */
 int eb200_scalar_mul_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_k, const uint32_t* d_key_idx,
