@@ -1080,6 +1080,29 @@ int run_sharded(size_t n, F&& fn) {
   return run_sharded_on(devs, nd, n, fn);
 }
 
+// Item i's range [off[i], off[i + 1]) of a variable-length input: not decreasing, and empty when the input is NULL.
+bool range_ok(const uint8_t* bytes, const uint64_t* off, size_t i) { return off[i + 1] >= off[i] && (bytes || !off[i + 1]); }
+// An address the staging copies can take for an input that is NULL because it is empty.
+const uint8_t* or_empty(const uint8_t* bytes) {
+  static const uint8_t none = 0;
+  return bytes ? bytes : &none;
+}
+constexpr auto every_item = [](size_t) { return true; };
+
+// The checks of an unkeyed host call, in order: a device, `supported` (the curve and public-key format; true for the
+// 25519 calls), n = 0, ptrs_ok, `unaccelerated` (a curve the call refuses after its pointer checks), item_ok(i) for
+// every item.  Then fn(c, lo, m) over the initialised devices (run_sharded).
+template <class ItemOk, class Fn>
+int host_run(bool supported, size_t n, bool ptrs_ok, ItemOk&& item_ok, Fn&& fn, bool unaccelerated = false) {
+  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (!supported) return EB200_ERR_UNSUPPORTED;
+  if (n == 0) return EB200_OK;
+  if (!ptrs_ok) return EB200_ERR_ARG;
+  if (unaccelerated) return EB200_ERR_UNSUPPORTED;
+  for (size_t i = 0; i < n; i++) if (!item_ok(i)) return EB200_ERR_ARG;
+  return run_sharded(n, fn);
+}
+
 // A device -> host copy; rows > 1: `rows` rows of `bytes`, `pitch` bytes apart on the device, packed on the host.
 // A NULL destination (an output the caller did not ask for) is skipped.
 struct OutSeg { void* dst; const void* src; size_t bytes; size_t rows = 1, pitch = 0; };
@@ -1360,27 +1383,20 @@ extern "C" {
 int eb200_ecdsa_verify_batch(int curve, size_t n, const uint8_t* e, const uint8_t* r,
                              const uint8_t* s, const uint8_t* pub, uint32_t pub_fmt,
                              uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (!curve_ok(curve) || !fmt_ok(pub_fmt)) return EB200_ERR_UNSUPPORTED;
-  if (n == 0) return EB200_OK;
-  if (!e || !r || !s || !pub || !status) return EB200_ERR_ARG;
   const size_t len = curve_len(curve), pb = pub_item_bytes(len, pub_fmt);
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
+  return host_run(curve_ok(curve) && fmt_ok(pub_fmt), n, e && r && s && pub && status, every_item, [&](Ctx& c, size_t lo, size_t m) {
     return verify_on(c, curve, m, e + lo * len, r + lo * len, s + lo * len, pub + lo * pb, pub_fmt, status + lo);
   });
 }
 
 int eb200_ecdsa_verify_batch_der(int curve, size_t n, const uint8_t* e, const uint8_t* sigs, const uint64_t* sig_off,
                                  const uint8_t* pub, uint32_t pub_fmt, uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (!curve_ok(curve) || !fmt_ok(pub_fmt)) return EB200_ERR_UNSUPPORTED;
-  if (n == 0) return EB200_OK;
-  if (!e || !sigs || !sig_off || !pub || !status) return EB200_ERR_ARG;
-  for (size_t i = 0; i < n; i++) if (sig_off[i + 1] < sig_off[i]) return EB200_ERR_ARG;
   const size_t len = curve_len(curve), pb = pub_item_bytes(len, pub_fmt);
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
-    return verify_der_on(c, curve, m, e + lo * len, sigs, sig_off + lo, pub + lo * pb, pub_fmt, status + lo);
-  });
+  return host_run(curve_ok(curve) && fmt_ok(pub_fmt), n, e && sigs && sig_off && pub && status,
+    [&](size_t i) { return range_ok(sigs, sig_off, i); },
+    [&](Ctx& c, size_t lo, size_t m) {
+      return verify_der_on(c, curve, m, e + lo * len, sigs, sig_off + lo, pub + lo * pb, pub_fmt, status + lo);
+    });
 }
 
 // ---- ECDSA public-key recovery ------------------------------------------------------------
@@ -1499,12 +1515,8 @@ static int mul_add_on(Ctx& c, int curve, size_t n, const uint8_t* k1, const uint
 
 static int mul_add_common(int curve, size_t n, const uint8_t* k1, const uint8_t* k2, const uint8_t* pts,
                           uint8_t* out_xy, uint8_t* status, bool derive = false) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
-  if (n == 0) return EB200_OK;
-  if (!k2 || !out_xy || !status || (k1 && !pts)) return EB200_ERR_ARG;
   const size_t len = curve_len(curve), ol = derive ? len : 2 * len;
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
+  return host_run(curve_ok(curve), n, k2 && out_xy && status && (!k1 || pts), every_item, [&](Ctx& c, size_t lo, size_t m) {
     return mul_add_on(c, curve, m, k1 ? k1 + lo * len : nullptr, k2 + lo * len, pts ? pts + lo * 2 * len : nullptr,
                       out_xy + lo * ol, status + lo, derive);
   });
@@ -1640,15 +1652,10 @@ extern "C" {
 
 int eb200_ecdsa_recover_batch(int curve, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
                               const uint8_t* recid, uint8_t* out_xy, uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
-  if (n == 0) return EB200_OK;
-  if (!e || !r || !s || !recid || !out_xy || !status) return EB200_ERR_ARG;
-  if (curve == EB200_CURVE_ED25519) return EB200_ERR_UNSUPPORTED;      // recoverPubKey over the Edwards preset is not accelerated
   const size_t len = curve_len(curve);
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
+  return host_run(curve_ok(curve), n, e && r && s && recid && out_xy && status, every_item, [&](Ctx& c, size_t lo, size_t m) {
     return recover_on(c, curve, m, e + lo * len, r + lo * len, s + lo * len, recid + lo, out_xy + lo * 2 * len, status + lo);
-  });
+  }, curve == EB200_CURVE_ED25519);      // recoverPubKey over the Edwards preset is not accelerated
 }
 
 int eb200_scalar_mul_batch(int curve, size_t n, const uint8_t* k, const uint8_t* points_xy, uint8_t* out_xy,
@@ -1670,58 +1677,48 @@ int eb200_mul_add_batch(int curve, size_t n, const uint8_t* k1, const uint8_t* k
 
 int eb200_ecdsa_sign_batch(int curve, size_t n, const uint8_t* e, const uint8_t* priv, uint32_t flags,
                            uint8_t* out_r, uint8_t* out_s, uint8_t* out_recid, uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
-  if (n == 0) return EB200_OK;
-  if (!e || !priv || !out_r || !out_s || !out_recid || !status) return EB200_ERR_ARG;
   const size_t len = curve_len(curve);
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
-    return sign_on(c, curve, m, e + lo * len, priv + lo * len, flags, out_r + lo * len, out_s + lo * len, out_recid + lo, status + lo);
-  });
+  return host_run(curve_ok(curve), n, e && priv && out_r && out_s && out_recid && status, every_item,
+    [&](Ctx& c, size_t lo, size_t m) {
+      return sign_on(c, curve, m, e + lo * len, priv + lo * len, flags, out_r + lo * len, out_s + lo * len, out_recid + lo,
+                     status + lo);
+    });
 }
 
 // EC.sign with options.k (ec/index.js:154-157): one attempt with the caller's nonces
 int eb200_ecdsa_sign_batch_k(int curve, size_t n, const uint8_t* e, const uint8_t* priv, const uint8_t* k, uint32_t flags,
                              uint8_t* out_r, uint8_t* out_s, uint8_t* out_recid, uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
-  if (n == 0) return EB200_OK;
-  if (!e || !priv || !k || !out_r || !out_s || !out_recid || !status) return EB200_ERR_ARG;
   const size_t len = curve_len(curve);
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
-    return sign_on(c, curve, m, e + lo * len, priv + lo * len, flags, out_r + lo * len, out_s + lo * len, out_recid + lo, status + lo,
-                   k + lo * len);
-  });
+  return host_run(curve_ok(curve), n, e && priv && k && out_r && out_s && out_recid && status, every_item,
+    [&](Ctx& c, size_t lo, size_t m) {
+      return sign_on(c, curve, m, e + lo * len, priv + lo * len, flags, out_r + lo * len, out_s + lo * len, out_recid + lo,
+                     status + lo, k + lo * len);
+    });
 }
 
 // EC.sign with options.pers (ec/index.js:143-151; the bytes after persEnc decoding, shared by the batch)
 int eb200_ecdsa_sign_batch_pers(int curve, size_t n, const uint8_t* e, const uint8_t* priv, const uint8_t* pers, size_t pers_len,
                                 uint32_t flags, uint8_t* out_r, uint8_t* out_s, uint8_t* out_recid, uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
-  if (n == 0) return EB200_OK;
-  if (!e || !priv || !out_r || !out_s || !out_recid || !status || (pers_len && !pers) || pers_len > (1u << 20)) return EB200_ERR_ARG;
-  static const uint8_t none = 0;
-  const uint8_t* pp = pers_len ? pers : &none;
+  const uint8_t* pp = or_empty(pers_len ? pers : nullptr);
   const size_t len = curve_len(curve);
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
-    return sign_on(c, curve, m, e + lo * len, priv + lo * len, flags, out_r + lo * len, out_s + lo * len, out_recid + lo, status + lo,
-                   nullptr, pp, pers_len);
-  });
+  return host_run(curve_ok(curve), n,
+    e && priv && out_r && out_s && out_recid && status && (pers || !pers_len) && pers_len <= (1u << 20), every_item,
+    [&](Ctx& c, size_t lo, size_t m) {
+      return sign_on(c, curve, m, e + lo * len, priv + lo * len, flags, out_r + lo * len, out_s + lo * len, out_recid + lo,
+                     status + lo, nullptr, pp, pers_len);
+    });
 }
 
 // EC.genKeyPair({entropy, pers}) (ec/index.js:55-79)
 int eb200_ec_keygen_batch(int curve, size_t n, const uint8_t* entropy, size_t entropy_len, const uint8_t* pers, size_t pers_len,
                           uint8_t* out_priv, uint8_t* out_pub_xy, uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
-  if (n == 0) return EB200_OK;
-  if (!entropy || !entropy_len || !out_priv || !status || (pers_len && !pers) || pers_len > (1u << 20) || entropy_len > (1u << 16)) return EB200_ERR_ARG;
   const size_t len = curve_len(curve);
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
-    return keygen_on(c, curve, m, entropy + lo * entropy_len, entropy_len, pers_len ? pers : nullptr, pers_len,
-                     out_priv + lo * len, out_pub_xy ? out_pub_xy + lo * 2 * len : nullptr, status + lo);
-  });
+  return host_run(curve_ok(curve), n,
+    entropy && entropy_len && out_priv && status && (pers || !pers_len) && pers_len <= (1u << 20) && entropy_len <= (1u << 16),
+    every_item, [&](Ctx& c, size_t lo, size_t m) {
+      return keygen_on(c, curve, m, entropy + lo * entropy_len, entropy_len, pers_len ? pers : nullptr, pers_len,
+                       out_priv + lo * len, out_pub_xy ? out_pub_xy + lo * 2 * len : nullptr, status + lo);
+    });
 }
 
 // ---- EdDSA (ed25519) verify ---------------------------------------------------------------
@@ -1880,10 +1877,7 @@ extern "C" {
 
 int eb200_eddsa_verify_batch(size_t n, const uint8_t* R, const uint8_t* S, const uint8_t* A, const uint8_t* h,
                              uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!R || !S || !A || !h || !status) return EB200_ERR_ARG;
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
+  return host_run(true, n, R && S && A && h && status, every_item, [&](Ctx& c, size_t lo, size_t m) {
     return eddsa_on(c, m, R + 32 * lo, S + 32 * lo, A + 32 * lo, h + 32 * lo, nullptr, nullptr, status + lo);
   });
 }
@@ -1891,29 +1885,20 @@ int eb200_eddsa_verify_batch(size_t n, const uint8_t* R, const uint8_t* S, const
 // EdDSA verify from raw messages: SHA-512 on the GPU (SURVEY 8f row 3), then the same verify kernel.
 int eb200_eddsa_verify_batch_msgs(size_t n, const uint8_t* R, const uint8_t* S, const uint8_t* A,
                                   const uint8_t* msgs, const uint64_t* msg_off, uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!R || !S || !A || !msg_off || !status || (!msgs && msg_off[n])) return EB200_ERR_ARG;
-  for (size_t i = 0; i < n; i++) if (msg_off[i + 1] < msg_off[i]) return EB200_ERR_ARG;
-  static const uint8_t none = 0;
-  const uint8_t* mp = msgs ? msgs : &none;
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
-    return eddsa_on(c, m, R + 32 * lo, S + 32 * lo, A + 32 * lo, nullptr, mp, msg_off + lo, status + lo);
-  });
+  return host_run(true, n, R && S && A && msg_off && status, [&](size_t i) { return range_ok(msgs, msg_off, i); },
+    [&](Ctx& c, size_t lo, size_t m) {
+      return eddsa_on(c, m, R + 32 * lo, S + 32 * lo, A + 32 * lo, nullptr, or_empty(msgs), msg_off + lo, status + lo);
+    });
 }
 
 // EDDSA.prototype.sign (eddsa/index.js:34-44) for keys given as 32-byte secrets (eddsa.keyFromSecret)
 int eb200_eddsa_sign_batch(size_t n, const uint8_t* secrets, const uint8_t* msgs, const uint64_t* msg_off,
                            uint8_t* out_sig, uint8_t* out_pub, uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!secrets || !msg_off || !out_sig || !status || (!msgs && msg_off[n])) return EB200_ERR_ARG;
-  for (size_t i = 0; i < n; i++) if (msg_off[i + 1] < msg_off[i]) return EB200_ERR_ARG;
-  static const uint8_t none = 0;
-  const uint8_t* mp = msgs ? msgs : &none;
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
-    return eddsa_sign_on(c, m, secrets + 32 * lo, mp, msg_off + lo, out_sig + 64 * lo, out_pub ? out_pub + 32 * lo : nullptr, status + lo);
-  });
+  return host_run(true, n, secrets && msg_off && out_sig && status, [&](size_t i) { return range_ok(msgs, msg_off, i); },
+    [&](Ctx& c, size_t lo, size_t m) {
+      return eddsa_sign_on(c, m, secrets + 32 * lo, or_empty(msgs), msg_off + lo, out_sig + 64 * lo,
+                           out_pub ? out_pub + 32 * lo : nullptr, status + lo);
+    });
 }
 
 // ---- curve25519 ECDH derive -------------------------------------------------------------------
@@ -1927,20 +1912,14 @@ int eb200_x25519_derive_batch_dev(size_t n, const uint8_t* d_priv, const uint8_t
 }
 
 int eb200_x25519_derive_batch(size_t n, const uint8_t* priv, const uint8_t* pubx, uint8_t* out, uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!priv || !pubx || !out || !status) return EB200_ERR_ARG;
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
+  return host_run(true, n, priv && pubx && out && status, every_item, [&](Ctx& c, size_t lo, size_t m) {
     return x25519_on(c, m, priv + 32 * lo, pubx + 32 * lo, out + 32 * lo, status + lo, true);
   });
 }
 
 // Montgomery-curve Point.mul (mont.js:130-153): x(k * P) for x-only points, k any 256-bit integer, no validation
 int eb200_x25519_mul_batch(size_t n, const uint8_t* k, const uint8_t* px, uint8_t* out_x, uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!k || !px || !out_x || !status) return EB200_ERR_ARG;
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
+  return host_run(true, n, k && px && out_x && status, every_item, [&](Ctx& c, size_t lo, size_t m) {
     return x25519_on(c, m, k + 32 * lo, px + 32 * lo, out_x + 32 * lo, status + lo, false);
   });
 }
@@ -2172,16 +2151,11 @@ extern "C" {
 
 int eb200_ecdsa_recovery_param_batch(int curve, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
                                      const uint8_t* q_xy, uint8_t* out_recid, uint8_t* status) {
-  if (!eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (!curve_ok(curve)) return EB200_ERR_UNSUPPORTED;
-  if (n == 0) return EB200_OK;
-  if (!e || !r || !s || !q_xy || !out_recid || !status) return EB200_ERR_ARG;
-  if (curve == EB200_CURVE_ED25519) return EB200_ERR_UNSUPPORTED;      // cofactor 8: the one-multiplication identity fails
   const size_t len = curve_len(curve);
-  return run_sharded(n, [&](Ctx& c, size_t lo, size_t m) {
+  return host_run(curve_ok(curve), n, e && r && s && q_xy && out_recid && status, every_item, [&](Ctx& c, size_t lo, size_t m) {
     return recovery_param_on(c, curve, m, e + lo * len, r + lo * len, s + lo * len, q_xy + lo * 2 * len, out_recid + lo,
                              status + lo);
-  });
+  }, curve == EB200_CURVE_ED25519);      // cofactor 8: the one-multiplication identity fails
 }
 
 }  // extern "C"
@@ -2255,20 +2229,45 @@ int keyset_build_on(Ctx& c, eb200_keyset* ks, const uint8_t* pub, uint8_t* key_s
     {{key_status, d.kst, m}}, {}, true);
 }
 
-// Keyed verify of one block on one device of the set, chunked like verify_on.
-int verify_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
-                    const u32* key_idx, uint8_t* status) {
-  const int curve = ks->curve;
-  const KeysetDev& d = ks->dev[c.device];
-  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
-  int rc = ensure_table(c, curve);
+// Workspace of one keyed_verify_launches block of n items: the prep words and the inversion scratch, as ws_layout places
+// them (no per-item table).
+size_t keyed_verify_ws_bytes(int curve, size_t n) { return ws_layout(curve, n).qtab; }
+
+// The launches of one keyed verify block whose inputs are on the device: the unchanged prep kernel of the set's curve,
+// then keyed main (between ev0 and ev1) and keyed replay.  base: keyed_verify_ws_bytes(curve, m) of workspace.
+int keyed_verify_launches(Ctx& c, int curve, size_t m, const KeysetDev& d, const uint8_t* e, const uint8_t* r, const uint8_t* s,
+                          const u32* idx, uint8_t* base, uint8_t* status, Launch& L, cudaEvent_t ev0, cudaEvent_t ev1) {
+  const WsLayout W = ws_layout(curve, m);
+  u32 *ws = (u32*)(base + W.ws), *scratch = (u32*)(base + W.scratch);
+  const u32* replay = nullptr;
+  int rc = with_curve(curve, [&](auto cv) {
+    typedef decltype(cv) T;
+    if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;
+    else if constexpr (is_k256<T>) {
+      L(k256_prep_kernel, batch_blocks(m, k256_prep_batch(m)), 128, m, e, r, s, ws, scratch, k256_prep_batch(m));
+      replay = c.replay_tab;
+    } else {
+      typedef typename T::C C;
+      L(sw_prep_kernel<C>, batch_blocks(m, SW<C>::BATCH), 128, m, e, r, s, ws, scratch);
+      replay = c.sw_replay_tab[curve];
+    }
+    return L.rc;
+  });
   if (rc) return rc;
+  const KeyedVerifyArgs a{e, r, s, idx, status, ws, c.gtab[curve], replay};
+  cudaError_t err = keyset_verify_launch(curve, m, d, a, L.st, ev0, ev1, &L.count);
+  return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_verify_launch");
+}
+
+// Keyed verify of one block on one device of the set, chunked like verify_on.  Launches per chunk: keyed_verify_launches.
+int verify_keyed_on(Ctx& c, const KeysetDev& d, int curve, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
+                    const u32* key_idx, uint8_t* status) {
+  int rc;
   const size_t len = curve_len(curve);
   const ChunkPlan P = make_plan(n);
   const size_t idx_bytes = align256(n * 4);
   if ((rc = grow(&c.d_in, &c.d_in_cap, idx_bytes + align256(n * 3 * len) + 1024))) return rc;
-  const WsLayout W = ws_layout(curve, P.max_m);
-  const size_t ws_slot = W.qtab;                    // prep words and the inversion scratch; no per-item table
+  const size_t ws_slot = keyed_verify_ws_bytes(curve, P.max_m);
   if ((rc = grow(&c.d_ws, &c.d_ws_cap, (P.chunks > 1 ? 2 : 1) * ws_slot))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
   u32* d_idx = (u32*)c.d_in;
@@ -2282,27 +2281,8 @@ int verify_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, 
       return 4;
     },
     [&](size_t lo, size_t m, Launch& L, int slot, int k) {
-      u32* ws = (u32*)(c.d_ws + (size_t)slot * ws_slot + W.ws);
-      u32* scratch = (u32*)(c.d_ws + (size_t)slot * ws_slot + W.scratch);
-      const u32* replay = nullptr;
-      int rc2 = with_curve(curve, [&](auto cv) {
-        typedef decltype(cv) T;
-        if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;
-        else if constexpr (is_k256<T>) {
-          L(k256_prep_kernel, batch_blocks(m, k256_prep_batch(m)), 128, m, d_e + lo * len, d_r + lo * len, d_s + lo * len, ws,
-            scratch, k256_prep_batch(m));
-          replay = c.replay_tab;
-        } else {
-          typedef typename T::C C;
-          L(sw_prep_kernel<C>, batch_blocks(m, SW<C>::BATCH), 128, m, d_e + lo * len, d_r + lo * len, d_s + lo * len, ws, scratch);
-          replay = c.sw_replay_tab[curve];
-        }
-        return L.rc;
-      });
-      if (rc2) return rc2;
-      const KeyedVerifyArgs a{d_e + lo * len, d_r + lo * len, d_s + lo * len, d_idx + lo, c.d_status + lo, ws, c.gtab[curve], replay};
-      cudaError_t err = keyset_verify_launch(curve, m, d, a, L.st, c.ev_k0[k], c.ev_k1[k], &L.count);
-      return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_verify_launch");
+      return keyed_verify_launches(c, curve, m, d, d_e + lo * len, d_r + lo * len, d_s + lo * len, d_idx + lo,
+                                   c.d_ws + (size_t)slot * ws_slot, c.d_status + lo, L, c.ev_k0[k], c.ev_k1[k]);
     },
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {status + lo, c.d_status + lo, m};
@@ -2310,42 +2290,19 @@ int verify_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, 
     });
 }
 
-// The unchanged prep kernel of the set's curve on L's stream (ws / scratch as ws_layout places them), and the curve's
-// replay table for keyset_verify_launch.
-int keyed_verify_prep(Ctx& c, int curve, size_t m, const uint8_t* d_e, const uint8_t* d_r, const uint8_t* d_s, u32* ws,
-                      u32* scratch, Launch& L, const u32** replay) {
-  return with_curve(curve, [&](auto cv) {
-    typedef decltype(cv) T;
-    if constexpr (is_ed25519<T>) return EB200_ERR_UNSUPPORTED;
-    else if constexpr (is_k256<T>) {
-      L(k256_prep_kernel, batch_blocks(m, k256_prep_batch(m)), 128, m, d_e, d_r, d_s, ws, scratch, k256_prep_batch(m));
-      *replay = c.replay_tab;
-    } else {
-      typedef typename T::C C;
-      L(sw_prep_kernel<C>, batch_blocks(m, SW<C>::BATCH), 128, m, d_e, d_r, d_s, ws, scratch);
-      *replay = c.sw_replay_tab[curve];
-    }
-    return L.rc;
-  });
-}
-
 // The launches of one keyed DER verify block whose inputs are on the device: the keyed DER decode (der + off[i] is item
-// i's encoding), or with `pre` the screened one (pre: the index-and-range screen's verdicts), then prep, keyed main
-// (between ev0 and ev1), keyed replay and verdict merge.  idx: the key indices the set may be addressed with; r, s
-// (m x len) and vd (m bytes) the decoded halves and verdicts; ws, scratch as ws_layout places them.
+// i's encoding), or with `pre` the screened one (pre: the index-and-range screen's verdicts), then keyed_verify_launches
+// and the verdict merge.  idx: the key indices the set may be addressed with; r, s (m x len) and vd (m bytes) the decoded
+// halves and verdicts; base: keyed_verify_ws_bytes(curve, m) of workspace.
 int keyed_der_launches(Ctx& c, int curve, size_t m, const KeysetDev& d, const uint8_t* e, const uint8_t* der,
                        const unsigned long long* off, const u32* idx, const uint8_t* pre, uint8_t* r, uint8_t* s, uint8_t* vd,
-                       u32* ws, u32* scratch, uint8_t* status, Launch& L, cudaEvent_t ev0, cudaEvent_t ev1) {
+                       uint8_t* base, uint8_t* status, Launch& L, cudaEvent_t ev0, cudaEvent_t ev1) {
   const u32 len = (u32)curve_len(curve);
   cudaError_t err = pre ? keyset_der_decode_screened_launch(m, len, pre, der, off, idx, d, r, s, vd, L.st, &L.count)
                         : keyset_der_decode_launch(m, len, der, off, idx, d, r, s, vd, L.st, &L.count);
   if (err != cudaSuccess) return cuda_fail(err, pre ? "keyset_der_decode_screened_launch" : "keyset_der_decode_launch");
-  const u32* replay = nullptr;
-  int rc = keyed_verify_prep(c, curve, m, e, r, s, ws, scratch, L, &replay);
+  int rc = keyed_verify_launches(c, curve, m, d, e, r, s, idx, base, status, L, ev0, ev1);
   if (rc) return rc;
-  const KeyedVerifyArgs a{e, r, s, idx, status, ws, c.gtab[curve], replay};
-  if ((err = keyset_verify_launch(curve, m, d, a, L.st, ev0, ev1, &L.count)) != cudaSuccess)
-    return cuda_fail(err, "keyset_verify_launch");
   if ((err = keyset_verdict_merge_launch(m, vd, status, L.st, &L.count)) != cudaSuccess)
     return cuda_fail(err, "keyset_verdict_merge_launch");
   return EB200_OK;
@@ -2354,21 +2311,16 @@ int keyed_der_launches(Ctx& c, int curve, size_t m, const KeysetDev& d, const ui
 // Keyed verify of DER signatures, one block on one device of the set, chunked like verify_keyed_on; the variable-length
 // segments as eddsa_sign_keyed_on stages them (sig_off points at this block's first offset, offsets absolute).
 // Launches per chunk: keyed_der_launches without a screen.
-int verify_keyed_der_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* sigs, const uint64_t* sig_off,
-                        const u32* key_idx, uint8_t* status) {
-  const int curve = ks->curve;
-  const KeysetDev& d = ks->dev[c.device];
-  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
-  int rc = ensure_table(c, curve);
-  if (rc) return rc;
+int verify_keyed_der_on(Ctx& c, const KeysetDev& d, int curve, size_t n, const uint8_t* e, const uint8_t* sigs,
+                        const uint64_t* sig_off, const u32* key_idx, uint8_t* status) {
+  int rc;
   const size_t len = curve_len(curve);
   const ChunkPlan P = make_plan(n);
   const size_t sig_bytes = (size_t)(sig_off[n] - sig_off[0]);
   const size_t off_bytes = align256((n + 1) * 8);
   const size_t base = align256(n * 4) + align256(n * 3 * len) + align256(n);   // key_idx | e, r, s | verdicts
   if ((rc = grow(&c.d_in, &c.d_in_cap, base + off_bytes + align256(sig_bytes + 1)))) return rc;
-  const WsLayout W = ws_layout(curve, P.max_m);
-  const size_t ws_slot = W.qtab;                    // prep words and the inversion scratch; no per-item table
+  const size_t ws_slot = keyed_verify_ws_bytes(curve, P.max_m);
   if ((rc = grow(&c.d_ws, &c.d_ws_cap, (P.chunks > 1 ? 2 : 1) * ws_slot))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
   u32* d_idx = (u32*)c.d_in;
@@ -2385,11 +2337,9 @@ int verify_keyed_der_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t*
       return 4;
     },
     [&](size_t lo, size_t m, Launch& L, int slot, int k) {
-      u32* ws = (u32*)(c.d_ws + (size_t)slot * ws_slot + W.ws);
-      u32* scratch = (u32*)(c.d_ws + (size_t)slot * ws_slot + W.scratch);
       return keyed_der_launches(c, curve, m, d, d_e + lo * len, d_sig - sig_off[0], d_off + lo, d_idx + lo, nullptr,
-                                d_r + lo * len, d_s + lo * len, d_vd + lo, ws, scratch, c.d_status + lo, L, c.ev_k0[k],
-                                c.ev_k1[k]);
+                                d_r + lo * len, d_s + lo * len, d_vd + lo, c.d_ws + (size_t)slot * ws_slot, c.d_status + lo, L,
+                                c.ev_k0[k], c.ev_k1[k]);
     },
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {status + lo, c.d_status + lo, m};
@@ -2410,10 +2360,10 @@ KeyedDevWs keyed_dev_ws(size_t n, size_t body) {
   return L;
 }
 
-// Workspace of one keyed mul / mulAdd / derive or getKeyRecoveryParam launch of n items: prep words | inversion scratch
-// (as ws_layout places them) | Jacobian results (3 x limbs x n words; recovery parameter: Y, Z, 2 x limbs x n).
+// Workspace of one keyed_mul_launches or keyed_rp_launches block of n items: prep words | inversion scratch (as
+// ws_layout places them) | Jacobian results (3 x limbs x n words; recovery parameter: Y, Z, 2 x limbs x n).
 size_t keyed_mul_ws_bytes(int curve, size_t n) {
-  return align256(ws_layout(curve, n).qtab + 3 * (size_t)keyset_geom(curve).limbs * n * 4);
+  return align256(keyed_verify_ws_bytes(curve, n) + 3 * (size_t)keyset_geom(curve).limbs * n * 4);
 }
 
 // eb200_ecdsa_verify_batch_keyed_der_dev keeps the decoded r, s (len bytes each) and the index-and-range screen's verdict
@@ -2459,13 +2409,9 @@ int keyed_mul_launches(Ctx& c, int curve, size_t m, const KeysetDev& d, const ui
 // k1 == NULL: k2 times the key (derive: x only, and an off-curve key is THROW_NOT_VALIDATED instead of replayed);
 // else k1 G + k2 times the key.  Launches per chunk: keyed_mul_launches.  derive: the private scalars, their digit
 // words and the Jacobian results are cleared on the chunk's stream behind its kernels, as x25519_on does.
-int mul_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* k1, const uint8_t* k2, const u32* key_idx,
+int mul_keyed_on(Ctx& c, const KeysetDev& d, int curve, size_t n, const uint8_t* k1, const uint8_t* k2, const u32* key_idx,
                  uint8_t* out, uint8_t* status, bool derive) {
-  const int curve = ks->curve;
-  const KeysetDev& d = ks->dev[c.device];
-  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
-  int rc = ensure_table(c, curve);
-  if (rc) return rc;
+  int rc;
   const size_t len = curve_len(curve), ol = derive ? len : 2 * len;
   const ChunkPlan P = make_plan(n);
   const size_t idx_bytes = align256(n * 4), k_bytes = align256(n * len);
@@ -2502,7 +2448,7 @@ int mul_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* k1, co
 
 // The launches of one keyed getKeyRecoveryParam block whose inputs are on the device: the unkeyed recovery-parameter
 // prep (recovery_param.cu), keyed main (between ev0 and ev1), recid normalisation, cold (keyset_recovery_param.cu).
-// base: the prep words, inversion scratch and Y, Z as recovery_param_keyed_on places them.
+// base: keyed_mul_ws_bytes(curve, m) of workspace (Y, Z in its Jacobian-result region).
 int keyed_rp_launches(Ctx& c, int curve, size_t m, const KeysetDev& d, const uint8_t* e, const uint8_t* r, const uint8_t* s,
                       const u32* idx, uint8_t* base, uint8_t* recid, uint8_t* status, Launch& L, cudaEvent_t ev0,
                       cudaEvent_t ev1) {
@@ -2518,19 +2464,14 @@ int keyed_rp_launches(Ctx& c, int curve, size_t m, const KeysetDev& d, const uin
 
 // Keyed getKeyRecoveryParam of one block on one device of the set, chunked like mul_keyed_on.  Launches per chunk:
 // keyed_rp_launches.
-int recovery_param_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r, const uint8_t* s,
-                            const u32* key_idx, uint8_t* out_recid, uint8_t* status) {
-  const int curve = ks->curve;
-  const KeysetDev& d = ks->dev[c.device];
-  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
-  int rc = ensure_table(c, curve);
-  if (rc) return rc;
-  const size_t len = curve_len(curve), limbs = (size_t)keyset_geom(curve).limbs;
+int recovery_param_keyed_on(Ctx& c, const KeysetDev& d, int curve, size_t n, const uint8_t* e, const uint8_t* r,
+                            const uint8_t* s, const u32* key_idx, uint8_t* out_recid, uint8_t* status) {
+  int rc;
+  const size_t len = curve_len(curve);
   const ChunkPlan P = make_plan(n);
   const size_t idx_bytes = align256(n * 4);
   if ((rc = grow(&c.d_in, &c.d_in_cap, idx_bytes + align256(n * 3 * len) + n + 256))) return rc;
-  const WsLayout W = ws_layout(curve, P.max_m);
-  const size_t ws_slot = align256(W.qtab + 2 * limbs * P.max_m * 4);   // prep words | inversion scratch | Y, Z
+  const size_t ws_slot = keyed_mul_ws_bytes(curve, P.max_m);
   if ((rc = grow(&c.d_ws, &c.d_ws_cap, (P.chunks > 1 ? 2 : 1) * ws_slot))) return rc;
   if ((rc = grow(&c.d_status, &c.d_status_cap, n))) return rc;
   u32* d_idx = (u32*)c.d_in;
@@ -2574,14 +2515,35 @@ int ed_keyset_build_on(Ctx& c, eb200_keyset* ks, const uint8_t* A, uint8_t* key_
     {{key_status, d.kst, m}}, {}, true);
 }
 
+// The launches of one keyed EdDSA verify block whose inputs are on the device.  msg_off != NULL (raw messages, m + 1
+// offsets relative to msgs): the keys' raw bytes gathered into A and h = SHA512(R || A || M) mod n into h first, by the
+// screened hash (keyset_forms.cu) when verdict != NULL; then the keyed verify between ev0 and ev1.
+int keyed_eddsa_verify_launches(Ctx& c, size_t m, const KeysetDev& d, const uint8_t* R, const uint8_t* S, uint8_t* h,
+                                uint8_t* A, const uint8_t* msgs, const u64* msg_off, const u32* idx, const uint8_t* verdict,
+                                uint8_t* status, Launch& L, cudaEvent_t ev0, cudaEvent_t ev1) {
+  cudaError_t err;
+  if (msg_off) {
+    if ((err = ed_keyset_gather_launch(m, d, idx, A, L.st, &L.count)) != cudaSuccess) return cuda_fail(err, "ed_keyset_gather_launch");
+    if (verdict) {
+      if ((err = keyset_ed_hash_screened_launch(m, verdict, R, A, msgs, msg_off, h, L.st, &L.count)) != cudaSuccess)
+        return cuda_fail(err, "keyset_ed_hash_screened_launch");
+    } else {
+      L(ed25519_hash_kernel, blocks128(m), 128, m, R, A, msgs, msg_off, h);
+      if (L.rc) return L.rc;
+    }
+  }
+  CK(cudaEventRecord(ev0, L.st));
+  if ((err = ed_keyset_verify_launch(m, d, R, S, h, idx, c.gtab[EB200_CURVE_ED25519], status, L.st, &L.count)) != cudaSuccess)
+    return cuda_fail(err, "ed_keyset_verify_launch");
+  CK(cudaEventRecord(ev1, L.st));
+  return EB200_OK;
+}
+
 // Keyed EdDSA verify of one block on one device of the set, chunked like eddsa_on.  h == NULL: raw messages (msg_off
-// points at this block's first offset, offsets absolute); the keys' raw bytes are gathered and hashed on the GPU.
-int eddsa_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* R, const uint8_t* S, const uint8_t* h,
+// points at this block's first offset, offsets absolute).  Launches per chunk: keyed_eddsa_verify_launches.
+int eddsa_keyed_on(Ctx& c, const KeysetDev& d, size_t n, const uint8_t* R, const uint8_t* S, const uint8_t* h,
                    const uint8_t* msgs, const uint64_t* msg_off, const u32* key_idx, uint8_t* status) {
-  const KeysetDev& d = ks->dev[c.device];
-  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
-  int rc = ensure_table(c, EB200_CURVE_ED25519);
-  if (rc) return rc;
+  int rc;
   const ChunkPlan P = make_plan(n);
   size_t mbytes = h ? 0 : (size_t)(msg_off[n] - msg_off[0]);
   size_t off_bytes = h ? 0 : (n + 1) * sizeof(uint64_t);
@@ -2592,7 +2554,6 @@ int eddsa_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* R, c
   u32* didx = (u32*)(dA + 32 * n);
   uint64_t* doff = (uint64_t*)(c.d_in + base);
   uint8_t* dm = c.d_in + base + align256(off_bytes);
-  const u32* gt = c.gtab[EB200_CURVE_ED25519];
   return run_chunked(c, P,
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {dR + 32 * lo, R + 32 * lo, 32 * m};
@@ -2604,19 +2565,9 @@ int eddsa_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* R, c
       return 5;
     },
     [&](size_t lo, size_t m, Launch& L, int, int k) {
-      cudaError_t err;
-      if (!h) {
-        if ((err = ed_keyset_gather_launch(m, d, didx + lo, dA + 32 * lo, L.st, &L.count)) != cudaSuccess)
-          return cuda_fail(err, "ed_keyset_gather_launch");
-        L(ed25519_hash_kernel, blocks128(m), 128, m, dR + 32 * lo, dA + 32 * lo, dm - msg_off[0], doff + lo, dh + 32 * lo);
-        if (L.rc) return L.rc;
-      }
-      CK(cudaEventRecord(c.ev_k0[k], L.st));
-      if ((err = ed_keyset_verify_launch(m, d, dR + 32 * lo, dS + 32 * lo, dh + 32 * lo, didx + lo, gt, c.d_status + lo, L.st,
-                                         &L.count)) != cudaSuccess)
-        return cuda_fail(err, "ed_keyset_verify_launch");
-      CK(cudaEventRecord(c.ev_k1[k], L.st));
-      return EB200_OK;
+      return keyed_eddsa_verify_launches(c, m, d, dR + 32 * lo, dS + 32 * lo, dh + 32 * lo, dA + 32 * lo,
+                                         h ? nullptr : dm - msg_off[0], h ? nullptr : doff + lo, didx + lo, nullptr,
+                                         c.d_status + lo, L, c.ev_k0[k], c.ev_k1[k]);
     },
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {status + lo, c.d_status + lo, m};
@@ -2643,14 +2594,25 @@ int ed_signset_build_on(Ctx& c, eb200_keyset* ks, const uint8_t* secrets, uint8_
     {{out_pub, d.xy, 32 * m}}, {{dsec, 32 * m}}, true);   // secrets do not stay in the shared buffer
 }
 
+// The launches of one keyed EdDSA sign block whose inputs are on the device (msg_off: m + 1 offsets relative to msgs):
+// ed_signset_sign_launch, or its screened form (keyset_forms.cu) when verdict != NULL, with the main kernels between ev0
+// and ev1; then the nonces r are cleared from ws (ed_signset_ws_bytes(m) bytes).
+int keyed_eddsa_sign_launches(Ctx& c, size_t m, const KeysetDev& d, const uint8_t* msgs, const u64* msg_off, const u32* idx,
+                              const uint8_t* verdict, uint8_t* ws, uint8_t* sig, Launch& L, cudaEvent_t ev0, cudaEvent_t ev1) {
+  const u32* gt = c.gtab[EB200_CURVE_ED25519];
+  cudaError_t err =
+      verdict ? keyset_ss_sign_screened_launch(m, verdict, d, msgs, msg_off, idx, gt, (u32*)ws, sig, L.st, ev0, ev1, &L.count)
+              : ed_signset_sign_launch(m, d, msgs, msg_off, idx, gt, (u32*)ws, sig, L.st, ev0, ev1, &L.count);
+  if (err != cudaSuccess) return cuda_fail(err, verdict ? "keyset_ss_sign_screened_launch" : "ed_signset_sign_launch");
+  CK(cudaMemsetAsync(ws + ed_signset_nonce_offset(m), 0, ed_signset_nonce_bytes(m), L.st));   // the nonces r
+  return EB200_OK;
+}
+
 // Keyed EdDSA sign of one block on one device of the set, chunked like eddsa_keyed_on (msg_off points at this block's
-// first offset, offsets absolute).  Each chunk's nonces r are cleared from the workspace behind its kernels.
-int eddsa_sign_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* msgs, const uint64_t* msg_off,
+// first offset, offsets absolute).  Launches per chunk: keyed_eddsa_sign_launches.
+int eddsa_sign_keyed_on(Ctx& c, const KeysetDev& d, size_t n, const uint8_t* msgs, const uint64_t* msg_off,
                         const u32* key_idx, uint8_t* sig) {
-  const KeysetDev& d = ks->dev[c.device];
-  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a key pointer of another device
-  int rc = ensure_table(c, EB200_CURVE_ED25519);
-  if (rc) return rc;
+  int rc;
   const ChunkPlan P = make_plan(n);
   const size_t mbytes = (size_t)(msg_off[n] - msg_off[0]);
   const size_t off_bytes = (n + 1) * sizeof(uint64_t);
@@ -2662,7 +2624,6 @@ int eddsa_sign_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t*
   u32* didx = (u32*)(dsig + 64 * n);
   uint64_t* doff = (uint64_t*)(c.d_in + base);
   uint8_t* dm = c.d_in + base + align256(off_bytes);
-  const u32* gt = c.gtab[EB200_CURVE_ED25519];
   return run_chunked(c, P,
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {didx + lo, key_idx + lo, 4 * m};
@@ -2671,12 +2632,8 @@ int eddsa_sign_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t*
       return 3;
     },
     [&](size_t lo, size_t m, Launch& L, int slot, int k) {
-      uint8_t* ws = c.d_ws + (size_t)slot * ws_slot;
-      cudaError_t err = ed_signset_sign_launch(m, d, dm - msg_off[0], doff + lo, didx + lo, gt, (u32*)ws, dsig + 64 * lo, L.st,
-                                               c.ev_k0[k], c.ev_k1[k], &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "ed_signset_sign_launch");
-      CK(cudaMemsetAsync(ws + ed_signset_nonce_offset(m), 0, ed_signset_nonce_bytes(m), L.st));   // the nonces r
-      return EB200_OK;
+      return keyed_eddsa_sign_launches(c, m, d, dm - msg_off[0], doff + lo, didx + lo, nullptr, c.d_ws + (size_t)slot * ws_slot,
+                                       dsig + 64 * lo, L, c.ev_k0[k], c.ev_k1[k]);
     },
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {sig + 64 * lo, dsig + 64 * lo, 64 * m};
@@ -2706,13 +2663,21 @@ int x25519_keyset_build_on(Ctx& c, eb200_keyset* ks, const uint8_t* pubx, uint8_
     {{key_status, d.kst, m}}, {}, true);
 }
 
-// Keyed curve25519 derive of one block on one device of the set, chunked like mul_keyed_on.  Launches per chunk: keyed
-// main, normalisation.  The private scalars and the workspace that holds the per-item results are cleared on the
-// chunk's stream behind its kernels.
-int x25519_derive_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8_t* priv, const u32* key_idx, uint8_t* out,
+// The launches of one keyed curve25519 derive block whose inputs are on the device: keyed main (between ev0 and ev1) and
+// normalisation; then the private scalars k and the per-item results in ws (x25519_keyset_ws_bytes(m) bytes) are cleared.
+int keyed_x25519_launches(size_t m, const KeysetDev& d, uint8_t* k, const u32* idx, uint8_t* ws, uint8_t* out, uint8_t* status,
+                          Launch& L, cudaEvent_t ev0, cudaEvent_t ev1) {
+  cudaError_t err = x25519_keyset_derive_launch(m, d, k, idx, (u32*)ws, out, status, L.st, ev0, ev1, &L.count);
+  if (err != cudaSuccess) return cuda_fail(err, "x25519_keyset_derive_launch");
+  CK(cudaMemsetAsync(k, 0, 32 * m, L.st));                           // the private scalars
+  CK(cudaMemsetAsync(ws, 0, x25519_keyset_ws_bytes(m), L.st));       // the per-item results
+  return EB200_OK;
+}
+
+// Keyed curve25519 derive of one block on one device of the set, chunked like mul_keyed_on.  Launches per chunk:
+// keyed_x25519_launches.
+int x25519_derive_keyed_on(Ctx& c, const KeysetDev& d, size_t n, const uint8_t* priv, const u32* key_idx, uint8_t* out,
                            uint8_t* status) {
-  const KeysetDev& d = ks->dev[c.device];
-  if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
   int rc;
   const ChunkPlan P = make_plan(n);
   const size_t idx_bytes = align256(n * 4), k_bytes = align256(n * 32);
@@ -2729,13 +2694,8 @@ int x25519_derive_keyed_on(Ctx& c, const eb200_keyset* ks, size_t n, const uint8
       return 2;
     },
     [&](size_t lo, size_t m, Launch& L, int slot, int k) {
-      uint8_t* ws = c.d_ws + (size_t)slot * ws_slot;
-      cudaError_t err = x25519_keyset_derive_launch(m, d, d_k + 32 * lo, d_idx + lo, (u32*)ws, d_out + 32 * lo, c.d_status + lo,
-                                                    L.st, c.ev_k0[k], c.ev_k1[k], &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "x25519_keyset_derive_launch");
-      CK(cudaMemsetAsync(d_k + 32 * lo, 0, 32 * m, L.st));              // the private scalars
-      CK(cudaMemsetAsync(ws, 0, x25519_keyset_ws_bytes(m), L.st));      // the per-item results
-      return EB200_OK;
+      return keyed_x25519_launches(m, d, d_k + 32 * lo, d_idx + lo, c.d_ws + (size_t)slot * ws_slot, d_out + 32 * lo,
+                                   c.d_status + lo, L, c.ev_k0[k], c.ev_k1[k]);
     },
     [&](size_t lo, size_t m, Seg* seg) {
       seg[0] = {out + 32 * lo, d_out + 32 * lo, 32 * m};
@@ -2793,7 +2753,7 @@ int keyset_create_on_devices(eb200_keyset* ks, eb200_keyset** out, Build&& build
   *out = ks;
   return EB200_OK;
 }
-// ---- device-pointer forms of the keyed calls ---------------------------------------------------------------------------
+// ---- argument checks and dispatch of the keyed calls -------------------------------------------------------------------
 // The kinds of set the keyed calls take.
 enum KeyedKind { KK_ECDSA, KK_ED_PUBLIC, KK_ED_SIGNING, KK_X25519 };
 bool keyed_kind_is(const eb200_keyset* ks, KeyedKind k) {
@@ -2804,10 +2764,35 @@ bool keyed_kind_is(const eb200_keyset* ks, KeyedKind k) {
     default: return ks->curve == EB200_CURVE_CURVE25519;
   }
 }
+// The fixed-base table the calls on a set of this kind use (0: none).
+int keyed_table_curve(const eb200_keyset* ks, KeyedKind kind) {
+  return kind == KK_ECDSA ? ks->curve : kind == KK_X25519 ? 0 : EB200_CURVE_ED25519;
+}
+
+// The checks of a keyed host call, in order: the set's kind, its lifetime, n = 0, ptrs_ok, then for every item its key
+// index and item_ok(i).  Then fn(c, d, lo, m) for the blocks of the batch, sharded over the set's devices, with d the
+// set's copy on c's device and the kind's fixed-base table loaded.
+template <class ItemOk, class Fn>
+int keyed_host_run(const eb200_keyset* ks, KeyedKind kind, size_t n, const u32* key_idx, bool ptrs_ok, ItemOk&& item_ok,
+                   Fn&& fn) {
+  if (!ks || !keyed_kind_is(ks, kind)) return EB200_ERR_ARG;
+  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
+  if (n == 0) return EB200_OK;
+  if (!ptrs_ok || !key_idx) return EB200_ERR_ARG;
+  for (size_t i = 0; i < n; i++) if (key_idx[i] >= ks->m || !item_ok(i)) return EB200_ERR_ARG;
+  const int table = keyed_table_curve(ks, kind);
+  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
+    const KeysetDev& d = ks->dev[c.device];
+    if (!d.tab) return EB200_ERR_NOT_INIT;           // never a table pointer of another device
+    int rc;
+    if (table && (rc = ensure_table(c, table))) return rc;
+    return fn(c, d, lo, m);
+  });
+}
 
 // Body bytes of the workspace (keyed_dev_ws) of the device-pointer calls a set takes, n items:
 //   ECDSA sets: keyed_mul_ws_bytes -- mul / mulAdd / derive and getKeyRecoveryParam as their host forms place it in
-//     each chunk's slot, the keyed verify its prep words and inversion scratch at the start;
+//     each chunk's slot, the keyed verify its keyed_verify_ws_bytes at the start;
 //   EdDSA sets: gathered key bytes (32 n, raw messages only) | h (32 n: the hash, or the screened copies of h);
 //   signing sets: ed_signset_ws_bytes, the sign launch's workspace;
 //   curve25519 sets: screened private scalars (32 n) | x25519_keyset_ws_bytes, the derive launch's workspace.
@@ -2832,12 +2817,34 @@ int keyed_dev_run(const eb200_keyset* ks, KeyedKind kind, size_t n, bool ptrs_ok
   if (!owner) return EB200_ERR_NOT_INIT;
   const KeysetDev& d = ks->dev[owner->device];
   if (!d.tab) return EB200_ERR_ARG;                // an initialised device that does not hold this set
-  const int table = kind == KK_ECDSA ? ks->curve : kind == KK_X25519 ? 0 : EB200_CURVE_ED25519;
   const KeyedDevWs Lw = keyed_dev_ws(n, 0);
   uint8_t* base = (uint8_t*)d_workspace;
-  return run_dev(d_status, table, stream, [&](Ctx& c, Launch& L) {
+  return run_dev(d_status, keyed_table_curve(ks, kind), stream, [&](Ctx& c, Launch& L) {
     return run(c, L, d, (u32*)(base + Lw.idx), base + Lw.verdict, base + Lw.prep);
   });
+}
+
+// The keyed device-pointer calls put a screen in front of their host form's launch function and a verdict merge behind
+// it; these return the CUDA error of a failed one.
+int index_screen(const eb200_keyset* ks, size_t n, const uint32_t* d_key_idx, u32* idx, uint8_t* vd, Launch& L) {
+  cudaError_t err = keyset_index_screen_launch(n, d_key_idx, ks->m, idx, vd, L.st, &L.count);
+  return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_index_screen_launch");
+}
+int range_screen(const eb200_keyset* ks, size_t n, const uint32_t* d_key_idx, const uint64_t* d_off, uint64_t len, u32* idx,
+                 uint8_t* vd, Launch& L) {
+  cudaError_t err = keyset_index_range_screen_launch(n, d_key_idx, ks->m, d_off, len, idx, vd, L.st, &L.count);
+  return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_index_range_screen_launch");
+}
+int scalar_screen(const eb200_keyset* ks, size_t n, const uint32_t* d_key_idx, const uint8_t* d_k, bool big_endian, u32* idx,
+                  uint8_t* k, uint8_t* vd, Launch& L) {
+  cudaError_t err = keyset_index_scalar_screen_launch(n, d_key_idx, ks->m, d_k, big_endian, idx, k, vd, L.st, &L.count);
+  return err == cudaSuccess ? EB200_OK : cuda_fail(err, "keyset_index_scalar_screen_launch");
+}
+// ol == 0: the verdicts replace the statuses; else they also zero the screened items' ol-byte rows of out.
+int verdict_merge(size_t n, const uint8_t* vd, uint8_t* d_status, uint8_t* out, u32 ol, Launch& L) {
+  cudaError_t err = ol ? keyset_verdict_merge_out_launch(n, vd, d_status, out, ol, L.st, &L.count)
+                       : keyset_verdict_merge_launch(n, vd, d_status, L.st, &L.count);
+  return err == cudaSuccess ? EB200_OK : cuda_fail(err, ol ? "keyset_verdict_merge_out_launch" : "keyset_verdict_merge_launch");
 }
 
 // Keyed mul / mulAdd / derive with device pointers: index screen, keyed_mul_launches, merge; derive clears the digit
@@ -2848,15 +2855,25 @@ int mul_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_k1, const u
     [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
       const int curve = ks->curve;
       const size_t ol = derive ? curve_len(curve) : 2 * curve_len(curve);
-      cudaError_t err = keyset_index_screen_launch(n, d_key_idx, ks->m, idx, vd, L.st, &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_screen_launch");
-      int rc = keyed_mul_launches(c, curve, n, d, d_k1, d_k2, idx, body, d_out, d_status, derive, L, c.ev[EV_MAIN_BEGIN],
-                                  c.ev[EV_MAIN_END]);
-      if (rc) return rc;
-      if ((err = keyset_verdict_merge_out_launch(n, vd, d_status, d_out, (u32)ol, L.st, &L.count)) != cudaSuccess)
-        return cuda_fail(err, "keyset_verdict_merge_out_launch");
+      int rc;
+      if ((rc = index_screen(ks, n, d_key_idx, idx, vd, L)) ||
+          (rc = keyed_mul_launches(c, curve, n, d, d_k1, d_k2, idx, body, d_out, d_status, derive, L, c.ev[EV_MAIN_BEGIN],
+                                   c.ev[EV_MAIN_END])) ||
+          (rc = verdict_merge(n, vd, d_status, d_out, (u32)ol, L)))
+        return rc;
       if (derive) CK(cudaMemsetAsync(body, 0, keyed_mul_ws_bytes(curve, n), L.st));   // digit words, Jacobian results
       return EB200_OK;
+    });
+}
+
+// The three keyed multiplication calls on host buffers: k1 == NULL (need_k1 false) is k2 times the key.
+int mul_keyed_host(const eb200_keyset* ks, size_t n, const uint8_t* k1, const uint8_t* k2, const uint32_t* key_idx,
+                   uint8_t* out, uint8_t* status, bool need_k1, bool derive) {
+  return keyed_host_run(ks, KK_ECDSA, n, key_idx, k2 && (k1 || !need_k1) && out && status, every_item,
+    [&](Ctx& c, const KeysetDev& d, size_t lo, size_t m) {
+      const size_t len = curve_len(ks->curve), ol = derive ? len : 2 * len;
+      return mul_keyed_on(c, d, ks->curve, m, k1 ? k1 + lo * len : nullptr, k2 + lo * len, key_idx + lo, out + lo * ol,
+                          status + lo, derive);
     });
 }
 }  // namespace
@@ -2908,33 +2925,26 @@ int eb200_keyset_destroy(eb200_keyset* ks) {
 
 int eb200_ecdsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r,
                                    const uint8_t* s, const uint32_t* key_idx, uint8_t* status) {
-  if (!ks || !keyset_geom(ks->curve).limbs) return EB200_ERR_ARG;      // an EdDSA or curve25519 set
-  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!e || !r || !s || !key_idx || !status) return EB200_ERR_ARG;
-  for (size_t i = 0; i < n; i++) if (key_idx[i] >= ks->m) return EB200_ERR_ARG;
-  const size_t len = curve_len(ks->curve);
-  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
-    return verify_keyed_on(c, ks, m, e + lo * len, r + lo * len, s + lo * len, key_idx + lo, status + lo);
-  });
+  return keyed_host_run(ks, KK_ECDSA, n, key_idx, e && r && s && status, every_item,
+    [&](Ctx& c, const KeysetDev& d, size_t lo, size_t m) {
+      const size_t len = curve_len(ks->curve);
+      return verify_keyed_on(c, d, ks->curve, m, e + lo * len, r + lo * len, s + lo * len, key_idx + lo, status + lo);
+    });
 }
 
 int eb200_ecdsa_verify_batch_keyed_der(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* sigs,
                                        const uint64_t* sig_off, const uint32_t* key_idx, uint8_t* status) {
-  if (!ks || !keyset_geom(ks->curve).limbs) return EB200_ERR_ARG;      // an EdDSA, signing or curve25519 set
-  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!e || !sigs || !sig_off || !key_idx || !status) return EB200_ERR_ARG;
-  for (size_t i = 0; i < n; i++) if (sig_off[i + 1] < sig_off[i] || key_idx[i] >= ks->m) return EB200_ERR_ARG;
-  const size_t len = curve_len(ks->curve);
-  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
-    return verify_keyed_der_on(c, ks, m, e + lo * len, sigs, sig_off + lo, key_idx + lo, status + lo);
-  });
+  return keyed_host_run(ks, KK_ECDSA, n, key_idx, e && sigs && sig_off && status,
+    [&](size_t i) { return range_ok(sigs, sig_off, i); },
+    [&](Ctx& c, const KeysetDev& d, size_t lo, size_t m) {
+      return verify_keyed_der_on(c, d, ks->curve, m, e + lo * curve_len(ks->curve), sigs, sig_off + lo, key_idx + lo,
+                                 status + lo);
+    });
 }
 
 size_t eb200_ecdsa_verify_keyed_workspace_bytes(const eb200_keyset* ks, size_t n) {
   if (!ks || !keyset_geom(ks->curve).limbs) return 0;
-  return keyed_dev_ws(n, ws_layout(ks->curve, n).qtab).total;
+  return keyed_dev_ws(n, keyed_verify_ws_bytes(ks->curve, n)).total;
 }
 
 int eb200_ecdsa_verify_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_e, const uint8_t* d_r,
@@ -2942,26 +2952,17 @@ int eb200_ecdsa_verify_batch_keyed_dev(const eb200_keyset* ks, size_t n, const u
                                        void* d_workspace, void* stream) {
   return keyed_dev_run(ks, KK_ECDSA, n, d_e && d_r && d_s && d_key_idx, d_status, d_workspace, stream,
     [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
-      const int curve = ks->curve;
-      const WsLayout W = ws_layout(curve, n);
-      u32* ws = (u32*)(body + W.ws);
-      u32* scratch = (u32*)(body + W.scratch);
-      cudaError_t err = keyset_index_screen_launch(n, d_key_idx, ks->m, idx, vd, L.st, &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_screen_launch");
-      const u32* replay = nullptr;
-      int rc = keyed_verify_prep(c, curve, n, d_e, d_r, d_s, ws, scratch, L, &replay);
-      if (rc) return rc;
-      const KeyedVerifyArgs a{d_e, d_r, d_s, idx, d_status, ws, c.gtab[curve], replay};
-      if ((err = keyset_verify_launch(curve, n, d, a, L.st, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END], &L.count)) != cudaSuccess)
-        return cuda_fail(err, "keyset_verify_launch");
-      if ((err = keyset_verdict_merge_launch(n, vd, d_status, L.st, &L.count)) != cudaSuccess)
-        return cuda_fail(err, "keyset_verdict_merge_launch");
-      return EB200_OK;
+      int rc;
+      if ((rc = index_screen(ks, n, d_key_idx, idx, vd, L)) ||
+          (rc = keyed_verify_launches(c, ks->curve, n, d, d_e, d_r, d_s, idx, body, d_status, L, c.ev[EV_MAIN_BEGIN],
+                                      c.ev[EV_MAIN_END])))
+        return rc;
+      return verdict_merge(n, vd, d_status, nullptr, 0, L);
     });
 }
 
-// workspace body (keyed_mul_ws_bytes): [prep words | inversion scratch | r (n x len) | s (n x len) | screen verdicts (n)],
-// the last three inside the Jacobian-result region (keyed_der_fits_jacobian)
+// workspace body (keyed_mul_ws_bytes): [keyed_verify_ws_bytes | r (n x len) | s (n x len) | screen verdicts (n)], the last
+// three inside the Jacobian-result region (keyed_der_fits_jacobian)
 int eb200_ecdsa_verify_batch_keyed_der_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_e, const uint8_t* d_sigs,
                                            uint64_t sigs_len, const uint64_t* d_sig_off, const uint32_t* d_key_idx,
                                            uint8_t* d_status, void* d_workspace, void* stream) {
@@ -2969,60 +2970,37 @@ int eb200_ecdsa_verify_batch_keyed_der_dev(const eb200_keyset* ks, size_t n, con
     [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
       const int curve = ks->curve;
       const size_t len = curve_len(curve);
-      const WsLayout W = ws_layout(curve, n);
-      uint8_t *r = body + W.qtab, *s = r + len * n, *pre = s + len * n;
-      cudaError_t err = keyset_index_range_screen_launch(n, d_key_idx, ks->m, d_sig_off, sigs_len, idx, pre, L.st, &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_range_screen_launch");
-      return keyed_der_launches(c, curve, n, d, d_e, d_sigs, (const unsigned long long*)d_sig_off, idx, pre,
-                                r, s, vd, (u32*)(body + W.ws), (u32*)(body + W.scratch), d_status, L, c.ev[EV_MAIN_BEGIN],
-                                c.ev[EV_MAIN_END]);
+      uint8_t *r = body + keyed_verify_ws_bytes(curve, n), *s = r + len * n, *pre = s + len * n;
+      int rc = range_screen(ks, n, d_key_idx, d_sig_off, sigs_len, idx, pre, L);
+      if (rc) return rc;
+      return keyed_der_launches(c, curve, n, d, d_e, d_sigs, (const unsigned long long*)d_sig_off, idx, pre, r, s, vd, body,
+                                d_status, L, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END]);
     });
 }
 
-}  // extern "C"
-
-// The three keyed multiplication calls: their argument checks, then the set's devices.
-static int mul_keyed_common(const eb200_keyset* ks, size_t n, const uint8_t* k1, const uint8_t* k2, const uint32_t* key_idx,
-                            uint8_t* out, uint8_t* status, bool need_k1, bool derive) {
-  if (!ks || !keyset_geom(ks->curve).limbs) return EB200_ERR_ARG;
-  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!k2 || (need_k1 && !k1) || !key_idx || !out || !status) return EB200_ERR_ARG;
-  for (size_t i = 0; i < n; i++) if (key_idx[i] >= ks->m) return EB200_ERR_ARG;
-  const size_t len = curve_len(ks->curve), ol = derive ? len : 2 * len;
-  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
-    return mul_keyed_on(c, ks, m, k1 ? k1 + lo * len : nullptr, k2 + lo * len, key_idx + lo, out + lo * ol, status + lo, derive);
-  });
-}
-
-extern "C" {
-
 int eb200_scalar_mul_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* k, const uint32_t* key_idx, uint8_t* out_xy,
                                  uint8_t* status) {
-  return mul_keyed_common(ks, n, nullptr, k, key_idx, out_xy, status, false, false);
+  return mul_keyed_host(ks, n, nullptr, k, key_idx, out_xy, status, false, false);
 }
 
 int eb200_mul_add_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* k1, const uint8_t* k2, const uint32_t* key_idx,
                               uint8_t* out_xy, uint8_t* status) {
-  return mul_keyed_common(ks, n, k1, k2, key_idx, out_xy, status, true, false);
+  return mul_keyed_host(ks, n, k1, k2, key_idx, out_xy, status, true, false);
 }
 
 int eb200_ecdh_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* priv, const uint32_t* key_idx, uint8_t* out_x,
                                   uint8_t* status) {
-  return mul_keyed_common(ks, n, nullptr, priv, key_idx, out_x, status, false, true);
+  return mul_keyed_host(ks, n, nullptr, priv, key_idx, out_x, status, false, true);
 }
 
 int eb200_ecdsa_recovery_param_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* e, const uint8_t* r,
                                            const uint8_t* s, const uint32_t* key_idx, uint8_t* out_recid, uint8_t* status) {
-  if (!ks || !keyset_geom(ks->curve).limbs) return EB200_ERR_ARG;
-  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!e || !r || !s || !key_idx || !out_recid || !status) return EB200_ERR_ARG;
-  for (size_t i = 0; i < n; i++) if (key_idx[i] >= ks->m) return EB200_ERR_ARG;
-  const size_t len = curve_len(ks->curve);
-  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
-    return recovery_param_keyed_on(c, ks, m, e + lo * len, r + lo * len, s + lo * len, key_idx + lo, out_recid + lo, status + lo);
-  });
+  return keyed_host_run(ks, KK_ECDSA, n, key_idx, e && r && s && out_recid && status, every_item,
+    [&](Ctx& c, const KeysetDev& d, size_t lo, size_t m) {
+      const size_t len = curve_len(ks->curve);
+      return recovery_param_keyed_on(c, d, ks->curve, m, e + lo * len, r + lo * len, s + lo * len, key_idx + lo,
+                                     out_recid + lo, status + lo);
+    });
 }
 
 int eb200_eddsa_keyset_create(size_t m, const uint8_t* A, uint32_t table_bits, uint8_t* key_status, eb200_keyset** out) {
@@ -3041,29 +3019,21 @@ int eb200_eddsa_keyset_create(size_t m, const uint8_t* A, uint32_t table_bits, u
 
 int eb200_eddsa_verify_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* R, const uint8_t* S, const uint8_t* h,
                                    const uint32_t* key_idx, uint8_t* status) {
-  if (!ks || ks->curve != EB200_CURVE_ED25519 || ks->kind != KS_PUBLIC) return EB200_ERR_ARG;
-  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!R || !S || !h || !key_idx || !status) return EB200_ERR_ARG;
-  for (size_t i = 0; i < n; i++) if (key_idx[i] >= ks->m || !ed_scalar_below_n(h + 32 * i)) return EB200_ERR_ARG;
-  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
-    return eddsa_keyed_on(c, ks, m, R + 32 * lo, S + 32 * lo, h + 32 * lo, nullptr, nullptr, key_idx + lo, status + lo);
-  });
+  return keyed_host_run(ks, KK_ED_PUBLIC, n, key_idx, R && S && h && status,
+    [&](size_t i) { return ed_scalar_below_n(h + 32 * i); },
+    [&](Ctx& c, const KeysetDev& d, size_t lo, size_t m) {
+      return eddsa_keyed_on(c, d, m, R + 32 * lo, S + 32 * lo, h + 32 * lo, nullptr, nullptr, key_idx + lo, status + lo);
+    });
 }
 
 int eb200_eddsa_verify_batch_keyed_msgs(const eb200_keyset* ks, size_t n, const uint8_t* R, const uint8_t* S,
                                         const uint8_t* msgs, const uint64_t* msg_off, const uint32_t* key_idx,
                                         uint8_t* status) {
-  if (!ks || ks->curve != EB200_CURVE_ED25519 || ks->kind != KS_PUBLIC) return EB200_ERR_ARG;
-  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!R || !S || !msg_off || !key_idx || !status || (!msgs && msg_off[n])) return EB200_ERR_ARG;
-  for (size_t i = 0; i < n; i++) if (msg_off[i + 1] < msg_off[i] || key_idx[i] >= ks->m) return EB200_ERR_ARG;
-  static const uint8_t none = 0;
-  const uint8_t* mp = msgs ? msgs : &none;
-  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
-    return eddsa_keyed_on(c, ks, m, R + 32 * lo, S + 32 * lo, nullptr, mp, msg_off + lo, key_idx + lo, status + lo);
-  });
+  return keyed_host_run(ks, KK_ED_PUBLIC, n, key_idx, R && S && msg_off && status,
+    [&](size_t i) { return range_ok(msgs, msg_off, i); },
+    [&](Ctx& c, const KeysetDev& d, size_t lo, size_t m) {
+      return eddsa_keyed_on(c, d, m, R + 32 * lo, S + 32 * lo, nullptr, or_empty(msgs), msg_off + lo, key_idx + lo, status + lo);
+    });
 }
 
 int eb200_eddsa_signing_set_create(size_t m, const uint8_t* secrets, uint8_t* out_pub, eb200_keyset** out) {
@@ -3077,17 +3047,12 @@ int eb200_eddsa_signing_set_create(size_t m, const uint8_t* secrets, uint8_t* ou
 
 int eb200_eddsa_sign_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* msgs, const uint64_t* msg_off,
                                  const uint32_t* key_idx, uint8_t* out_sig, uint8_t* status) {
-  if (!ks || ks->curve != EB200_CURVE_ED25519 || ks->kind != KS_SIGNING) return EB200_ERR_ARG;
-  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!msg_off || !key_idx || !out_sig || !status || (!msgs && msg_off[n])) return EB200_ERR_ARG;
-  for (size_t i = 0; i < n; i++) if (msg_off[i + 1] < msg_off[i] || key_idx[i] >= ks->m) return EB200_ERR_ARG;
-  static const uint8_t none = 0;
-  const uint8_t* mp = msgs ? msgs : &none;
-  int rc = run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
-    return eddsa_sign_keyed_on(c, ks, m, mp, msg_off + lo, key_idx + lo, out_sig + 64 * lo);
-  });
-  if (rc == EB200_OK) memset(status, EB200_ST_TRUE, n);         // the reference cannot fail here
+  int rc = keyed_host_run(ks, KK_ED_SIGNING, n, key_idx, msg_off && out_sig && status,
+    [&](size_t i) { return range_ok(msgs, msg_off, i); },
+    [&](Ctx& c, const KeysetDev& d, size_t lo, size_t m) {
+      return eddsa_sign_keyed_on(c, d, m, or_empty(msgs), msg_off + lo, key_idx + lo, out_sig + 64 * lo);
+    });
+  if (rc == EB200_OK && n) memset(status, EB200_ST_TRUE, n);         // the reference cannot fail here
   return rc;
 }
 
@@ -3107,19 +3072,12 @@ int eb200_x25519_keyset_create(size_t m, const uint8_t* pubx, uint32_t table_bit
 
 int eb200_x25519_derive_batch_keyed(const eb200_keyset* ks, size_t n, const uint8_t* priv, const uint32_t* key_idx,
                                     uint8_t* out_x, uint8_t* status) {
-  if (!ks || ks->curve != EB200_CURVE_CURVE25519) return EB200_ERR_ARG;
-  if (!ks->live || !eb200_device_count()) return EB200_ERR_NOT_INIT;
-  if (n == 0) return EB200_OK;
-  if (!priv || !key_idx || !out_x || !status) return EB200_ERR_ARG;
-  for (size_t i = 0; i < n; i++) if (key_idx[i] >= ks->m || !x25519_priv_below_n(priv + 32 * i)) return EB200_ERR_ARG;
-  return run_sharded_on(ks->devs, ks->ndev, n, [&](Ctx& c, size_t lo, size_t m) {
-    return x25519_derive_keyed_on(c, ks, m, priv + 32 * lo, key_idx + lo, out_x + 32 * lo, status + lo);
-  });
+  return keyed_host_run(ks, KK_X25519, n, key_idx, priv && out_x && status,
+    [&](size_t i) { return x25519_priv_below_n(priv + 32 * i); },
+    [&](Ctx& c, const KeysetDev& d, size_t lo, size_t m) {
+      return x25519_derive_keyed_on(c, d, m, priv + 32 * lo, key_idx + lo, out_x + 32 * lo, status + lo);
+    });
 }
-
-}  // extern "C"
-
-extern "C" {
 
 size_t eb200_keyset_dev_workspace_bytes(const eb200_keyset* ks, size_t n) {
   if (!ks) return 0;
@@ -3147,14 +3105,12 @@ int eb200_ecdsa_recovery_param_batch_keyed_dev(const eb200_keyset* ks, size_t n,
                                                uint8_t* d_status, void* d_workspace, void* stream) {
   return keyed_dev_run(ks, KK_ECDSA, n, d_e && d_r && d_s && d_key_idx && d_out_recid, d_status, d_workspace, stream,
     [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
-      cudaError_t err = keyset_index_screen_launch(n, d_key_idx, ks->m, idx, vd, L.st, &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_screen_launch");
-      int rc = keyed_rp_launches(c, ks->curve, n, d, d_e, d_r, d_s, idx, body, d_out_recid, d_status, L, c.ev[EV_MAIN_BEGIN],
-                                 c.ev[EV_MAIN_END]);
-      if (rc) return rc;
-      if ((err = keyset_verdict_merge_out_launch(n, vd, d_status, d_out_recid, 1, L.st, &L.count)) != cudaSuccess)
-        return cuda_fail(err, "keyset_verdict_merge_out_launch");
-      return EB200_OK;
+      int rc;
+      if ((rc = index_screen(ks, n, d_key_idx, idx, vd, L)) ||
+          (rc = keyed_rp_launches(c, ks->curve, n, d, d_e, d_r, d_s, idx, body, d_out_recid, d_status, L, c.ev[EV_MAIN_BEGIN],
+                                  c.ev[EV_MAIN_END])))
+        return rc;
+      return verdict_merge(n, vd, d_status, d_out_recid, 1, L);
     });
 }
 
@@ -3165,16 +3121,12 @@ int eb200_eddsa_verify_batch_keyed_dev(const eb200_keyset* ks, size_t n, const u
   return keyed_dev_run(ks, KK_ED_PUBLIC, n, d_R && d_S && d_h && d_key_idx, d_status, d_workspace, stream,
     [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
       uint8_t* h = body + align256(32 * n);
-      cudaError_t err = keyset_index_scalar_screen_launch(n, d_key_idx, ks->m, d_h, false, idx, h, vd, L.st, &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_scalar_screen_launch");
-      CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
-      if ((err = ed_keyset_verify_launch(n, d, d_R, d_S, h, idx, c.gtab[EB200_CURVE_ED25519], d_status, L.st, &L.count)) !=
-          cudaSuccess)
-        return cuda_fail(err, "ed_keyset_verify_launch");
-      CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
-      if ((err = keyset_verdict_merge_launch(n, vd, d_status, L.st, &L.count)) != cudaSuccess)
-        return cuda_fail(err, "keyset_verdict_merge_launch");
-      return EB200_OK;
+      int rc;
+      if ((rc = scalar_screen(ks, n, d_key_idx, d_h, false, idx, h, vd, L)) ||
+          (rc = keyed_eddsa_verify_launches(c, n, d, d_R, d_S, h, nullptr, nullptr, nullptr, idx, nullptr, d_status, L,
+                                            c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END])))
+        return rc;
+      return verdict_merge(n, vd, d_status, nullptr, 0, L);
     });
 }
 
@@ -3185,63 +3137,44 @@ int eb200_eddsa_verify_batch_keyed_msgs_dev(const eb200_keyset* ks, size_t n, co
   return keyed_dev_run(ks, KK_ED_PUBLIC, n, d_R && d_S && d_msg_off && d_key_idx && (d_msgs || !msgs_len), d_status,
                        d_workspace, stream,
     [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
-      uint8_t *A = body, *h = body + align256(32 * n);
-      cudaError_t err = keyset_index_range_screen_launch(n, d_key_idx, ks->m, d_msg_off, msgs_len, idx, vd, L.st, &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_range_screen_launch");
-      if ((err = ed_keyset_gather_launch(n, d, idx, A, L.st, &L.count)) != cudaSuccess)
-        return cuda_fail(err, "ed_keyset_gather_launch");
-      if ((err = keyset_ed_hash_screened_launch(n, vd, d_R, A, d_msgs, d_msg_off, h, L.st, &L.count)) != cudaSuccess)
-        return cuda_fail(err, "keyset_ed_hash_screened_launch");
-      CK(cudaEventRecord(c.ev[EV_MAIN_BEGIN], L.st));
-      if ((err = ed_keyset_verify_launch(n, d, d_R, d_S, h, idx, c.gtab[EB200_CURVE_ED25519], d_status, L.st, &L.count)) !=
-          cudaSuccess)
-        return cuda_fail(err, "ed_keyset_verify_launch");
-      CK(cudaEventRecord(c.ev[EV_MAIN_END], L.st));
-      if ((err = keyset_verdict_merge_launch(n, vd, d_status, L.st, &L.count)) != cudaSuccess)
-        return cuda_fail(err, "keyset_verdict_merge_launch");
-      return EB200_OK;
+      int rc;
+      if ((rc = range_screen(ks, n, d_key_idx, d_msg_off, msgs_len, idx, vd, L)) ||
+          (rc = keyed_eddsa_verify_launches(c, n, d, d_R, d_S, body + align256(32 * n), body, d_msgs, d_msg_off, idx, vd,
+                                            d_status, L, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END])))
+        return rc;
+      return verdict_merge(n, vd, d_status, nullptr, 0, L);
     });
 }
 
-// workspace body: the sign launch's (ed_signset_ws_bytes); its nonces are cleared behind the kernels, as
-// eddsa_sign_keyed_on clears them
+// workspace body: the sign launch's (ed_signset_ws_bytes)
 int eb200_eddsa_sign_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_msgs, uint64_t msgs_len,
                                      const uint64_t* d_msg_off, const uint32_t* d_key_idx, uint8_t* d_out_sig,
                                      uint8_t* d_status, void* d_workspace, void* stream) {
   return keyed_dev_run(ks, KK_ED_SIGNING, n, d_msg_off && d_key_idx && d_out_sig && (d_msgs || !msgs_len), d_status,
                        d_workspace, stream,
     [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
-      cudaError_t err = keyset_index_range_screen_launch(n, d_key_idx, ks->m, d_msg_off, msgs_len, idx, vd, L.st, &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_range_screen_launch");
-      if ((err = keyset_ss_sign_screened_launch(n, vd, d, d_msgs, d_msg_off, idx, c.gtab[EB200_CURVE_ED25519], (u32*)body,
-                                                d_out_sig, L.st, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END], &L.count)) !=
-          cudaSuccess)
-        return cuda_fail(err, "keyset_ss_sign_screened_launch");
+      int rc;
+      if ((rc = range_screen(ks, n, d_key_idx, d_msg_off, msgs_len, idx, vd, L)) ||
+          (rc = keyed_eddsa_sign_launches(c, n, d, d_msgs, d_msg_off, idx, vd, body, d_out_sig, L, c.ev[EV_MAIN_BEGIN],
+                                          c.ev[EV_MAIN_END])))
+        return rc;
       CK(cudaMemsetAsync(d_status, EB200_ST_TRUE, n, L.st));          // the reference cannot fail here
-      if ((err = keyset_verdict_merge_out_launch(n, vd, d_status, d_out_sig, 64, L.st, &L.count)) != cudaSuccess)
-        return cuda_fail(err, "keyset_verdict_merge_out_launch");
-      CK(cudaMemsetAsync(body + ed_signset_nonce_offset(n), 0, ed_signset_nonce_bytes(n), L.st));   // the nonces r
-      return EB200_OK;
+      return verdict_merge(n, vd, d_status, d_out_sig, 64, L);
     });
 }
 
-// workspace body: [screened private scalars (32 n) | the derive launch's (x25519_keyset_ws_bytes)], all cleared behind
-// the kernels
+// workspace body: [screened private scalars (32 n) | the derive launch's (x25519_keyset_ws_bytes)]
 int eb200_x25519_derive_batch_keyed_dev(const eb200_keyset* ks, size_t n, const uint8_t* d_priv, const uint32_t* d_key_idx,
                                         uint8_t* d_out_x, uint8_t* d_status, void* d_workspace, void* stream) {
   return keyed_dev_run(ks, KK_X25519, n, d_priv && d_key_idx && d_out_x, d_status, d_workspace, stream,
     [&](Ctx& c, Launch& L, const KeysetDev& d, u32* idx, uint8_t* vd, uint8_t* body) {
       uint8_t* k = body;
-      u32* ws = (u32*)(body + align256(32 * n));
-      cudaError_t err = keyset_index_scalar_screen_launch(n, d_key_idx, ks->m, d_priv, true, idx, k, vd, L.st, &L.count);
-      if (err != cudaSuccess) return cuda_fail(err, "keyset_index_scalar_screen_launch");
-      if ((err = x25519_keyset_derive_launch(n, d, k, idx, ws, d_out_x, d_status, L.st, c.ev[EV_MAIN_BEGIN], c.ev[EV_MAIN_END],
-                                             &L.count)) != cudaSuccess)
-        return cuda_fail(err, "x25519_keyset_derive_launch");
-      if ((err = keyset_verdict_merge_out_launch(n, vd, d_status, d_out_x, 32, L.st, &L.count)) != cudaSuccess)
-        return cuda_fail(err, "keyset_verdict_merge_out_launch");
-      CK(cudaMemsetAsync(body, 0, keyed_dev_body_bytes(ks, n), L.st));   // the scalars and the per-item results
-      return EB200_OK;
+      int rc;
+      if ((rc = scalar_screen(ks, n, d_key_idx, d_priv, true, idx, k, vd, L)) ||
+          (rc = keyed_x25519_launches(n, d, k, idx, body + align256(32 * n), d_out_x, d_status, L, c.ev[EV_MAIN_BEGIN],
+                                      c.ev[EV_MAIN_END])))
+        return rc;
+      return verdict_merge(n, vd, d_status, d_out_x, 32, L);
     });
 }
 

@@ -29,7 +29,8 @@ GTAB_DIMS = {
     0: (-5, -1, -1, -1), 1: (0, 13, 524288, 20), 2: (0, 20, 4096, 13), 3: (0, 30, 4096, 13), 4: (0, 18, 4096, 13),
     5: (-5, -1, -1, -1), 6: (0, 41, 4096, 13), 7: (0, 15, 4096, 13), 8: (0, 18, 4096, 13), 9: (-5, -1, -1, -1),
 }
-# return codes without a device (-3 ERR_ARG, -4 ERR_NOT_INIT, -5 ERR_UNSUPPORTED); nullK: NULL in argument K
+# return codes without a device (-3 ERR_ARG, -4 ERR_NOT_INIT, -5 ERR_UNSUPPORTED); nullK: NULL in argument K.  The
+# keyed calls get a NULL set here, which they refuse before they look for a device.
 NO_DEVICE = {
     "eb200_ecdsa_verify_batch": {"curve77": -4, "n0": -4, "null2": -4, "null3": -4, "null4": -4, "null5": -4, "fmt9": -4, "null7": -4},
     "eb200_ecdsa_verify_batch_der": {"curve77": -4, "n0": -4, "null2": -4, "null3": -4, "null4": -4, "null5": -4, "fmt9": -4, "null7": -4},
@@ -42,6 +43,8 @@ NO_DEVICE = {
                                     "null10": -4},
     "eb200_ec_keygen_batch": {"curve77": -4, "n0": -4, "null2": -4, "null4": -4, "null6": -4, "null7": -4, "null8": -4},
     "eb200_ecdsa_recover_batch": {"curve77": -4, "n0": -4, "null2": -4, "null3": -4, "null4": -4, "null5": -4, "null6": -4, "null7": -4},
+    "eb200_ecdsa_recovery_param_batch": {"curve77": -4, "n0": -4, "null2": -4, "null3": -4, "null4": -4, "null5": -4,
+                                         "null6": -4, "null7": -4},
     "eb200_scalar_mul_batch": {"curve77": -4, "n0": -4, "null2": -4, "null3": -4, "null4": -4, "null5": -4},
     "eb200_ecdh_derive_batch": {"curve77": -4, "n0": -4, "null2": -4, "null3": -3, "null4": -4, "null5": -4},
     "eb200_mul_add_batch": {"curve77": -4, "n0": -4, "null2": -3, "null3": -4, "null4": -3, "null5": -4, "null6": -4},
@@ -57,6 +60,36 @@ NO_DEVICE = {
     "eb200_curve_add_batch": {"desc_null": -4, "n0": -4, "null2": -4, "null3": -3, "null4": -4, "null5": -4},
     "eb200_curve_dbl_batch": {"desc_null": -4, "n0": -4, "null2": -4, "null3": -4, "null4": -4},
     "eb200_curve_validate_batch": {"desc_null": -4, "n0": -4, "null2": -4, "null3": -4},
+    "eb200_ecdsa_verify_batch_keyed": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3},
+    "eb200_ecdsa_verify_batch_keyed_der": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3},
+    "eb200_ecdsa_verify_batch_keyed_dev": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                           "null7": -3, "null8": -3},
+    "eb200_scalar_mul_batch_keyed": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3},
+    "eb200_mul_add_batch_keyed": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3},
+    "eb200_ecdh_derive_batch_keyed": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3},
+    "eb200_ecdsa_recovery_param_batch_keyed": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                               "null7": -3},
+    "eb200_eddsa_verify_batch_keyed": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3},
+    "eb200_eddsa_verify_batch_keyed_msgs": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                            "null7": -3},
+    "eb200_eddsa_sign_batch_keyed": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3},
+    "eb200_x25519_derive_batch_keyed": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3},
+    "eb200_ecdsa_verify_batch_keyed_der_dev": {"n0": -3, "null2": -3, "null3": -3, "null5": -3, "null6": -3, "null7": -3,
+                                               "null8": -3, "null9": -3},
+    "eb200_scalar_mul_batch_keyed_dev": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3, "null7": -3},
+    "eb200_mul_add_batch_keyed_dev": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3, "null7": -3,
+                                      "null8": -3},
+    "eb200_ecdh_derive_batch_keyed_dev": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3, "null7": -3},
+    "eb200_ecdsa_recovery_param_batch_keyed_dev": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                                   "null7": -3, "null8": -3, "null9": -3},
+    "eb200_eddsa_verify_batch_keyed_dev": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                           "null7": -3, "null8": -3},
+    "eb200_eddsa_verify_batch_keyed_msgs_dev": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null6": -3, "null7": -3,
+                                                "null8": -3, "null9": -3, "null10": -3},
+    "eb200_eddsa_sign_batch_keyed_dev": {"n0": -3, "null2": -3, "null4": -3, "null5": -3, "null6": -3, "null7": -3, "null8": -3,
+                                         "null9": -3},
+    "eb200_x25519_derive_batch_keyed_dev": {"n0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                            "null7": -3},
     "eb200_selftest_fe": {"curve77": -4, "n0": -4, "null3": -4, "null4": -4, "null5": -4},
     "eb200_selftest_gtab": {"curve77": -4, "null1": -4},
     "eb200_selftest_gtab_dims": {"curve77": -5, "null1": -3, "null2": -3, "null3": -3},

@@ -205,9 +205,50 @@ WITH_DEVICE = {
     "eb200_x25519_derive_batch": {"n0": 0, "null1": -3, "null2": -3, "null3": -3, "null4": -3},
     "eb200_x25519_derive_batch_dev": {"n0": 0, "null1": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -4},
     "eb200_x25519_mul_batch": {"n0": 0, "null1": -3, "null2": -3, "null3": -3, "null4": -3},
+    "eb200_ecdh_derive_batch_keyed": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "wrong_set": -3},
+    "eb200_ecdh_derive_batch_keyed_dev": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                          "null7": -4, "wrong_set": -3},
+    "eb200_ecdsa_recovery_param_batch": {"curve77": -5, "n0": 0, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                         "null7": -3},
+    "eb200_ecdsa_recovery_param_batch_keyed": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3,
+                                               "null6": -3, "null7": -3, "wrong_set": -3},
+    "eb200_ecdsa_recovery_param_batch_keyed_dev": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3,
+                                                   "null6": -3, "null7": -3, "null8": -3, "null9": -4, "wrong_set": -3},
+    "eb200_ecdsa_verify_batch_keyed": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                       "wrong_set": -3},
+    "eb200_ecdsa_verify_batch_keyed_der": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                           "wrong_set": -3},
+    "eb200_ecdsa_verify_batch_keyed_der_dev": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null5": -3, "null6": -3,
+                                               "null7": -3, "null8": -3, "null9": -4, "wrong_set": -3},
+    "eb200_ecdsa_verify_batch_keyed_dev": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                           "null7": -3, "null8": -4, "wrong_set": -3},
+    "eb200_eddsa_sign_batch_keyed": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                     "wrong_set": -3},
+    "eb200_eddsa_sign_batch_keyed_dev": {"n0": 0, "null0": -3, "null2": -3, "null4": -3, "null5": -3, "null6": -3, "null7": -3,
+                                         "null8": -3, "null9": -4, "wrong_set": -3},
+    "eb200_eddsa_verify_batch_keyed": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                       "wrong_set": -3},
+    "eb200_eddsa_verify_batch_keyed_dev": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                           "null7": -3, "null8": -4, "wrong_set": -3},
+    "eb200_eddsa_verify_batch_keyed_msgs": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3,
+                                            "null6": -3, "null7": -3, "wrong_set": -3},
+    "eb200_eddsa_verify_batch_keyed_msgs_dev": {"n0": 0, "null0": -3, "null10": -4, "null2": -3, "null3": -3, "null4": -3,
+                                                "null6": -3, "null7": -3, "null8": -3, "null9": -3, "wrong_set": -3},
+    "eb200_mul_add_batch_keyed": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                  "wrong_set": -3},
+    "eb200_mul_add_batch_keyed_dev": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                      "null7": -3, "null8": -4, "wrong_set": -3},
+    "eb200_scalar_mul_batch_keyed": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "wrong_set": -3},
+    "eb200_scalar_mul_batch_keyed_dev": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3, "null6": -3,
+                                         "null7": -4, "wrong_set": -3},
+    "eb200_x25519_derive_batch_keyed": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3,
+                                        "wrong_set": -3},
+    "eb200_x25519_derive_batch_keyed_dev": {"n0": 0, "null0": -3, "null2": -3, "null3": -3, "null4": -3, "null5": -3,
+                                            "null6": -3, "null7": -4, "wrong_set": -3},
 }
 # eb200_timing.launches after each call of launch_cases(): kernels launched per entry point x curve x mode
-# (curve ids as in the header; fmtF: public-key format; 262921 items and `chunked`: cut into chunks)
+# (curve ids as in the header; fmtF: public-key format; 262921 items and `chunked`: cut into chunks; *_keyed: against
+# sets of 16 keys, the ECDSA ones on the curve named)
 LAUNCHES = {
     "curve_add/p256": 1, "curve_add/p384": 1, "curve_add/p521": 1,
     "curve_dbl/p256": 1, "curve_dbl/p384": 1, "curve_dbl/p521": 1,
@@ -254,6 +295,19 @@ LAUNCHES = {
     "x25519_derive/256": 1, "x25519_derive/262921": 5,
     "x25519_derive_dev": 1,
     "x25519_mul/256": 1, "x25519_mul/262921": 5,
+    "derive_keyed/1/256": 4, "derive_keyed/1/262921": 20, "derive_keyed/2/256": 4, "derive_keyed/2/262921": 20,
+    "derive_keyed_dev/1": 6, "derive_keyed_dev/2": 6, "eddsa_sign_keyed/256": 3, "eddsa_sign_keyed/262921": 15,
+    "eddsa_sign_keyed_dev": 5, "eddsa_verify_keyed/256": 1, "eddsa_verify_keyed/262921": 5, "eddsa_verify_keyed_dev": 3,
+    "eddsa_verify_keyed_msgs/256": 3, "eddsa_verify_keyed_msgs/262921": 15, "eddsa_verify_keyed_msgs_dev": 5,
+    "mul_add_keyed/1/256": 4, "mul_add_keyed/1/262921": 20, "mul_add_keyed/2/256": 4, "mul_add_keyed/2/262921": 20,
+    "mul_add_keyed_dev/1": 6, "mul_add_keyed_dev/2": 6, "mul_keyed/1/256": 4, "mul_keyed/1/262921": 20,
+    "mul_keyed/2/256": 4, "mul_keyed/2/262921": 20, "mul_keyed_dev/1": 6, "mul_keyed_dev/2": 6,
+    "recovery_param_keyed/1/256": 4, "recovery_param_keyed/1/262921": 20, "recovery_param_keyed/2/256": 4,
+    "recovery_param_keyed/2/262921": 20, "recovery_param_keyed_dev/1": 6, "recovery_param_keyed_dev/2": 6,
+    "verify_keyed/1/256": 3, "verify_keyed/1/262921": 15, "verify_keyed/2/256": 3, "verify_keyed/2/262921": 15,
+    "verify_keyed_der/1/256": 5, "verify_keyed_der/1/262921": 25, "verify_keyed_der/2/256": 5,
+    "verify_keyed_der/2/262921": 25, "verify_keyed_der_dev/1": 6, "verify_keyed_der_dev/2": 6, "verify_keyed_dev/1": 5,
+    "verify_keyed_dev/2": 5, "x25519_derive_keyed/256": 2, "x25519_derive_keyed/262921": 10, "x25519_derive_keyed_dev": 4,
 }
 
 
